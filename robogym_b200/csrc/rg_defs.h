@@ -126,7 +126,7 @@ __device__ __forceinline__ void rg_stage_sync() {
 #define RG_NEL 64
 #endif
 #define RG_CON_STRIDE 24
-#define RG_CPRM 6           /* per-contact solver parameters: D, dim, B, K*imp*r, number of dofs, their sign bits (solimp[5] is staged there by the collision stage) */
+#define RG_CPRM 6           /* per-contact solver parameters: D, dim, first slot (rg_slot_col), unused, number of dofs, their sign bits (solimp[5] is staged there by the collision stage) */
 #ifndef RG_GRP
 #define RG_GRP 8           /* lanes that share one pair in the convex-convex narrow phase (rg_mpr_batch) */
 #endif
