@@ -92,7 +92,12 @@ int rg_model_name2id(const rg_model* m, const char* objtype, const char* name);
 const char* rg_model_id2name(const rg_model* m, const char* objtype, int id);   /* NULL when out of range; "" for an unnamed object */
 /* overwrite a model array (host float64 / int32 values, `count` elements) and re-upload it.  The upload is ordered on
  * `stream` (set_field: the legacy default stream): launches queued before it keep the old values.  The host buffers may be
- * reused as soon as the call returns.  Do not call it from two threads for the same model at once. */
+ * reused as soon as the call returns.  Do not call it from two threads for the same model at once.
+ * Besides the arrays of include/rg_model_fields.h, `name` may be "mesh_scale": [nmesh] uniform scale of every convex hull
+ * (1 at load; finite and > 0, else the call fails).  The narrow phase then uses the hull scaled by s about its frame origin --
+ * support point s v*, with v* the support vertex of the unscaled hull -- and scales the hull's bounding box of the OBB cull
+ * with it; geom_rbound (the broad phase) stays what the caller set, as in MuJoCo.  It is not part of the blob.  Editing
+ * "mesh_vert" also rebuilds what the narrow phase derives from it (the padded vertex copy it scans, the geom_aabb of mesh geoms). */
 int rg_model_set_field(rg_model* m, const char* name, const void* data, size_t count);
 int rg_model_set_field_async(rg_model* m, const char* name, const void* data, size_t count, void* stream);
 /* floats per environment of the RG_FIELD_DBG dump; bytes of shared memory per environment (one warp) */
@@ -116,7 +121,8 @@ int rg_batch_bind(rg_batch* b, int field, void* device_ptr);
  * sim.model.geom_friction / dof_damping / actuator_gainprm / opt_gravity / ... per env and per episode):
  * device_ptr is a float32 [nenv][count(name)] tensor that replaces the shared array `name` for each environment.
  * Up to RG_MAX_PARAM_OVERRIDES arrays; device_ptr == NULL removes the override.  body_pos rows of bodies attached
- * to the world must be given relative to rg_model_origin(). */
+ * to the world must be given relative to rg_model_origin().  "mesh_scale" ([nenv][nmesh], see rg_model_set_field) gives every
+ * environment its own hull sizes; its values must be finite and > 0 (not checked on the device). */
 int rg_batch_bind_param(rg_batch* b, const char* name, void* device_ptr);
 int rg_model_origin(const rg_model* m, float origin[3]);
 /* Work-ordered scheduling (default on; RG_BALANCE=0 in the environment turns it off at create): every launch records a

@@ -173,6 +173,7 @@ struct RgModel {
   const int* dof_xlvl;         /* the same lists restricted to the dofs that stay out of the constraint solver */
   const int* dof_sidx;         /* [2 nv]: solver position of every dof (or -1), then the dof at every solver position */
   const int* eqrow;            /* [neqrow]: equality id * 8 + row (weld: 6 rows, joint coupling: 1); row k is "virtual tendon" ntendon + k */
+  const float* mesh_scale;     /* [nmesh]: uniform scale of every hull (1 at load; model-wide or per-environment parameter) */
   const float* mesh_vert4;     /* [nmeshvert][4]: hull vertices padded to 16 bytes (one vector load each) */
   const unsigned short* pair_packed; /* [npair] geom1 | geom2 << 8 when ngeom <= 256 (staged in shared memory), else nullptr */
   float origin[3];             /* world translation applied at load so coordinates stay small in fp32 */
@@ -230,6 +231,7 @@ struct RgModelDev {
   RgArr<int> dof_xlvl;
   RgArr<int> dof_sidx;
   RgArr<int> eqrow;
+  RgArr<float> mesh_scale;
   RgArr<unsigned short> pair_packed;
   int has_pairs;
   const float* mesh_vert4;

@@ -101,6 +101,7 @@ __global__ void __launch_bounds__(RG_MAX_WARPS * 32, 1) rg_step_kernel(const __g
     RG_SETOFF(dof_xlvl)
     RG_SETOFF(dof_sidx)
     RG_SETOFF(eqrow)
+    RG_SETOFF(mesh_scale)
     RG_SETPTR(mesh_vert4)
     if (lane == 0) {
       sm->has_pairs = args.m.pair_packed != nullptr;
@@ -296,6 +297,7 @@ static void rg_wire_device_view(rg_model* mm) {
   RG_DEVPTR(dof_xlvl)
   RG_DEVPTR(dof_sidx)
   RG_DEVPTR(eqrow)
+  RG_DEVPTR(mesh_scale)
   RG_DEVPTR(mesh_vert4)
   if (mm->hm.view.pair_packed) RG_DEVPTR(pair_packed)
 #undef RG_DEVPTR
@@ -376,8 +378,13 @@ int rg_model_set_field_async(rg_model* mm, const char* name, const void* data, s
 #undef RG_DIM
 #undef RG_I
 #undef RG_F
+  const bool is_scale = !strcmp(name, "mesh_scale");   /* derived array of the engine, not a blob field */
+  if (is_scale) { hptr = (void*)m.mesh_scale; n = (size_t)m.nmesh; }
   if (!hptr) return rg_fail(-1, std::string("rg_model_set_field: unknown field ") + name);
   if (n != count) return rg_fail(-1, std::string("rg_model_set_field: size mismatch for ") + name);
+  if (is_scale)
+    for (size_t i = 0; i < n; i++)
+      if (!(((const double*)data)[i] > 0.0) || !isfinite(((const double*)data)[i])) return rg_fail(-1, "rg_model_set_field: mesh_scale must be finite and positive");
   if (isint) memcpy(hptr, data, 4 * n);
   else {
     const double* s = (const double*)data;
@@ -394,6 +401,27 @@ int rg_model_set_field_async(rg_model* mm, const char* name, const void* data, s
   /* stream-ordered: launches already queued on `stream` still see the old values, later ones the new; the host copy is
      pageable, so the runtime stages it before returning and `data` / the host arena may change right away */
   RG_CUDA(cudaMemcpyAsync(mm->d_arena + off, hptr, 4 * n, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  if (!strcmp(name, "mesh_vert")) {
+    /* what the narrow phase derives from the hulls follows them: the float4-padded copy it scans, and the geom-frame box of
+       every mesh geom that the OBB cull tests (the vertex bounding box, as the model compiler computes it) */
+    rg_host_pad_verts(m);
+    const size_t off4 = (const char*)m.mesh_vert4 - mm->hm.arena.data();
+    RG_CUDA(cudaMemcpyAsync(mm->d_arena + off4, m.mesh_vert4, 16 * (size_t)m.nmeshvert, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    const double* v = (const double*)data;
+    float* aabb = (float*)m.geom_aabb;
+    for (int g = 0; g < m.ngeom; g++) {
+      if (m.geom_type[g] != RG_GEOM_MESH) continue;
+      const int mid = m.geom_dataid[g], a = m.mesh_vertadr[mid], nvt = m.mesh_vertnum[mid];
+      for (int k = 0; k < 3 && nvt > 0; k++) {
+        double lo = v[3 * a + k], hi = lo;
+        for (int q = 1; q < nvt; q++) { lo = fmin(lo, v[3 * (a + q) + k]); hi = fmax(hi, v[3 * (a + q) + k]); }
+        aabb[6 * g + k] = (float)(0.5 * (lo + hi));
+        aabb[6 * g + 3 + k] = (float)(0.5 * (hi - lo));
+      }
+    }
+    const size_t offb = (const char*)m.geom_aabb - mm->hm.arena.data();
+    RG_CUDA(cudaMemcpyAsync(mm->d_arena + offb, m.geom_aabb, 24 * (size_t)m.ngeom, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  }
   return 0;
 }
 
@@ -513,6 +541,7 @@ int rg_batch_bind_param(rg_batch* b, const char* name, void* p) {
 #undef RG_F
 #undef RG_IB
 #undef RG_FB
+  if (!strcmp(name, "mesh_scale")) { off = (int)offsetof(RgModelDev, mesh_scale); cnt = m.nmesh; }
   if (off < 0) return rg_fail(-1, std::string("rg_batch_bind_param: not a (small) float model array: ") + name);
   int slot = -1;
   for (int i = 0; i < b->nover; i++) if (b->over_name[i] == name) slot = i;

@@ -24,6 +24,12 @@ struct RgHostModel {
 
 static inline size_t rg_align16(size_t x) { return (x + 15) & ~(size_t)15; }
 
+/* (re)build the float4-padded hull vertices the narrow phase reads from mesh_vert (at load, and after mesh_vert was edited) */
+static inline void rg_host_pad_verts(RgModel& m) {
+  float* v4 = (float*)m.mesh_vert4;
+  for (int k = 0; k < m.nmeshvert; k++) { v4[4 * k] = m.mesh_vert[3 * k]; v4[4 * k + 1] = m.mesh_vert[3 * k + 1]; v4[4 * k + 2] = m.mesh_vert[3 * k + 2]; v4[4 * k + 3] = 0.0f; }
+}
+
 static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, std::string& err) {
   const char* p = (const char*)blob;
   if (len < 12 || memcmp(p, "RGMODEL1", 8)) { err = "bad model blob magic"; return false; }
@@ -101,6 +107,7 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
   dst = rg_align16(dst); const size_t off_sidx = dst; dst += 4 * (2 * (size_t)m.nv);
   dst = rg_align16(dst); const size_t off_eqrow = dst; dst += 4 * (6 * (size_t)m.neq + 1);
   dst = rg_align16(dst); const size_t off_pairs = dst; if (m.ngeom <= 256) dst += 2 * (size_t)m.npair;
+  dst = rg_align16(dst); const size_t off_mscale = dst; dst += 4 * (size_t)m.nmesh;
   dst = rg_align16(dst);
   hm.small_bytes = dst;
   for (size_t i = first_big; i < names.size(); i++) { dst = rg_align16(dst); dstoff[i] = dst; dst += 4 * counts[i]; }
@@ -234,10 +241,15 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
   hm.offsets.push_back(off_xlvl);
   hm.offsets.push_back(off_sidx);
   hm.offsets.push_back(off_eqrow);
+  /* uniform hull scale: the narrow phase's support point of a mesh is mesh_scale * (arg-max vertex of the unscaled hull) */
+  float* mscale = (float*)(base + off_mscale);
+  for (int k = 0; k < m.nmesh; k++) mscale[k] = 1.0f;
+  m.mesh_scale = mscale;
+  hm.offsets.push_back(off_mscale);
   /* hull vertices padded to float4: the narrow phase scans a hull's vertices with one 16-byte load each */
   float* v4 = (float*)(base + off_v4);
-  for (int k = 0; k < m.nmeshvert; k++) { v4[4 * k] = m.mesh_vert[3 * k]; v4[4 * k + 1] = m.mesh_vert[3 * k + 1]; v4[4 * k + 2] = m.mesh_vert[3 * k + 2]; v4[4 * k + 3] = 0.0f; }
   m.mesh_vert4 = v4;
+  rg_host_pad_verts(m);
   m.pair_packed = nullptr;
   if (m.ngeom <= 256) {
     unsigned short* pk = (unsigned short*)(base + off_pairs);

@@ -78,12 +78,21 @@ def _check(rc):
         raise EngineError(lib().rg_last_error().decode())
 
 
+def check_mesh_scale(v):
+    """mesh_scale values must be finite and > 0: the narrow phase scales the arg-max vertex of the unscaled hull, which is
+    the scaled hull's support point only for a positive scale."""
+    a = np.asarray(v.detach().cpu() if hasattr(v, "detach") else v, dtype=np.float64)
+    if not (np.isfinite(a).all() and (a > 0).all()):
+        raise ValueError("mesh_scale must be finite and positive")
+
+
 class DeviceModel:
     """A compiled model uploaded to one GPU (rg_model)."""
 
     def __init__(self, blob, device=0):
         self.blob = bytes(blob)
         self.host = modelblob.unpack(self.blob)  # float64 host copy, source of truth for edits
+        self.mesh_scale = np.ones(self.host["nmesh"])  # engine-derived parameter (not in the blob): uniform scale per hull
         self.device = int(device)
         h = ctypes.c_void_p()
         _check(lib().rg_model_load(self.blob, len(self.blob), self.device, ctypes.byref(h)))
@@ -94,8 +103,11 @@ class DeviceModel:
 
     def set_field(self, name, values, stream=None):
         """Overwrite a model array (randomisers write e.g. geom_friction, dof_damping, opt_gravity).  The upload is ordered
-        on `stream` (a raw cudaStream_t; default: torch's current stream on the model's device when torch is loaded)."""
-        arr = self.host[name]
+        on `stream` (a raw cudaStream_t; default: torch's current stream on the model's device when torch is loaded).
+        `mesh_scale` ([nmesh], finite and > 0) scales every hull uniformly without touching mesh_vert."""
+        if name == "mesh_scale":
+            check_mesh_scale(values)
+        arr = self.mesh_scale if name == "mesh_scale" else self.host[name]
         arr[...] = np.asarray(values, dtype=arr.dtype).reshape(arr.shape)
         buf = np.ascontiguousarray(arr)
         if stream is None:
@@ -233,8 +245,11 @@ class BatchedSim:
         v = t.as_tensor(np.asarray(values, dtype=np.float64) if not t.is_tensor(values) else values).to(t.float64).reshape(rows, -1).clone()
         if idx is not None and name not in getattr(self, "_params", {}):
             raise EngineError(f"set_param({name}, idx=...): bind the full array first")
-        if v.shape[1] != m[name].size:
-            raise EngineError(f"set_param({name}): expected {m[name].size} values per environment, got {v.shape[1]}")
+        count = m["nmesh"] if name == "mesh_scale" else m[name].size     # mesh_scale: the engine's per-hull scale, not a blob array
+        if v.shape[1] != count:
+            raise EngineError(f"set_param({name}): expected {count} values per environment, got {v.shape[1]}")
+        if name == "mesh_scale":
+            check_mesh_scale(v)
         if name in ("body_pos", "geom_pos", "site_pos"):
             # keep the engine's fp32 world shift: bodies attached to the world, and geoms / sites attached to the world body
             o = (ctypes.c_float * 3)()

@@ -16,6 +16,7 @@ per-environment parameter rows (`BatchedSim.set_param` -> `rg_batch_bind_param`)
 | jnt_range + ctrlrange  | randomizations.RandomizedJointLimitWrapper (593-670)                         |
 | tendon_range           | randomizations.RandomizedTendonRangeWrapper (673-717)                        |
 | cube size              | cube.RandomizedCubeSizeWrapper (cube.py:12-52): x U(0.95, 1.05)              |
+| full cube size         | parametric.RandomizedPerpendicularCubeSizeWrapper (parametric.py:24-38): cubelet body_pos, named cubelet geom_rbound, cubelet hull mesh_scale x U(0.95, 1.05), then set_const on the device (FullCubeRandomizer(cube_size_range=...)) |
 | phasespace sites       | dactyl.RandomizedPhasespaceFingersWrapper (dactyl.py:14-60): + N(0, sigma) per site |
 | timestep (per step)    | randomizations.RandomizedTimestepWrapper (194-311)                           |
 | wind (per step)        | cube.RandomizedWindWrapper (cube.py:56-85)                                   |
@@ -300,16 +301,63 @@ class FullCubeRandomizer(LockedRandomizer):
     (body inertias, robot / cube friction, gravity, robot damping, Kp, joint limits, tendon ranges, phasespace marker offsets, per-step
     timestep, wind on `cube:middle`) plus `RandomizedFaceDampingWrapper` (wrappers/face.py:4-9: the damping of the cube's face-driver and
     cubelet joints times a log-uniform factor in [1/3, 3] per dof).  Cube friction applies to every named cube geom (25 cubelets + the core sphere)
-    (`RandomizedCubeFrictionWrapper` takes every geom whose name starts with "cube:").  NOT covered: `RandomizedPerpendicularCubeSizeWrapper`
-    -- its modifier rescales the cubelet MESH (envs/dactyl/common/mujoco_modifiers.py:55-66), and mesh vertices are shared by the whole
-    batch here; the cube keeps its nominal size."""
+    (`RandomizedCubeFrictionWrapper` takes every geom whose name starts with "cube:").
 
-    def __init__(self, m, names, rand, torch, device, dtype, hand_prefix="robot0:", cube_prefix="cube:"):
+    `cube_size_range=(lo, hi)` adds `RandomizedPerpendicularCubeSizeWrapper` (wrappers/parametric.py:24-38) with the edits of its
+    `PerpendicularCubeSizeModifier` (envs/dactyl/common/mujoco_modifiers.py:8-66): one s ~ U(lo, hi) per environment, drawn after every
+    other draw, scales the original `body_pos` of the 26 `cube:cubelet:*` bodies, the `geom_rbound` of the 25 NAMED cubelet geoms (the
+    reference leaves one cubelet geom unnamed, and its bounding sphere unscaled), and the cubelet hull `cube:rounded_cube` through the
+    engine's per-environment `mesh_scale` row.  Masses and inertias keep their values.  As the reference calls `set_constants()` after
+    its modifiers (cube_env.py:343-349), `apply()` then recomputes dof_invweight0 / body_invweight0 / tendon_invweight0 /
+    opt_meaninertia on the device (`BatchedSim.set_const`) from each environment's own rows: `BatchedConstants` assumes the shared model's
+    geometry.  `None` (default) leaves the cube at its nominal size and every row as without the argument."""
+
+    def __init__(self, m, names, rand, torch, device, dtype, hand_prefix="robot0:", cube_prefix="cube:", cube_size_range=None):
         super().__init__(m, names, rand, torch, device, dtype, hand_prefix, cube_prefix)
         jn = names["joint"]
         face_j = {j for j, nme in enumerate(jn) if nme is not None and (nme.startswith(cube_prefix + "cubelet:driver:") or nme.startswith(cube_prefix + "cubelet:rot"))}
         self.face_dofs = torch.as_tensor([d for d in range(m["nv"]) if int(m["dof_jntid"][d]) in face_j], dtype=torch.long, device=device)
+        self.cube_size_range = None if cube_size_range is None else (float(cube_size_range[0]), float(cube_size_range[1]))
+        if self.cube_size_range is not None:
+            lo, hi = self.cube_size_range
+            if not (0.0 < lo <= hi and math.isfinite(hi)):
+                raise ValueError(f"cube_size_range must satisfy 0 < low <= high < inf, got {cube_size_range}")
+            pre = cube_prefix + "cubelet:"
+            sel = lambda lst: torch.as_tensor([i for i, nme in enumerate(lst) if nme is not None and nme.startswith(pre)], dtype=torch.long, device=device)
+            self.cubelet_bodies = sel(names["body"])
+            self.cubelet_geoms = sel(names["geom"])
+            self.cube_mesh = names["mesh"].index(cube_prefix + "rounded_cube")
+            self.orig["body_pos"] = torch.as_tensor(np.asarray(m["body_pos"]), dtype=dtype, device=device).reshape(1, -1)
+            self.orig["mesh_scale"] = torch.ones(1, m["nmesh"], dtype=dtype, device=device)
 
     def _extra_rules(self, n, draw, out):
         damp = out["dof_damping"]
         damp[:, self.face_dofs] = damp[:, self.face_dofs] * draw("face_damping", lambda: self._logu(1 / 3.0, 3.0, n, int(self.face_dofs.numel())))
+
+    def sample(self, n, noises=None):
+        out = super().sample(n, noises)
+        if self.cube_size_range is None:
+            return out
+        nz = noises or {}
+        s = nz["cube_size"].to(self.dtype) if "cube_size" in nz else self.rand.uniform(*self.cube_size_range, n, 1)   # last draw of the episode
+        o = self.orig
+        bp = o["body_pos"].reshape(1, -1, 3).repeat(n, 1, 1)
+        bp[:, self.cubelet_bodies] = bp[:, self.cubelet_bodies] * s.reshape(n, 1, 1)
+        out["body_pos"] = bp.reshape(n, -1)
+        rb = o["geom_rbound"].repeat(n, 1)
+        rb[:, self.cubelet_geoms] = rb[:, self.cubelet_geoms] * s.reshape(n, 1)
+        out["geom_rbound"] = rb
+        ms = o["mesh_scale"].repeat(n, 1)
+        ms[:, self.cube_mesh] = s.reshape(n)
+        out["mesh_scale"] = ms
+        return out
+
+    def apply(self, sim, params, idx=None):
+        super().apply(sim, params, idx)
+        if self.cube_size_range is not None:
+            # set_constants() after the modifiers: the scaled cubelet offsets move the bodies' centres of mass
+            mask = None
+            if idx is not None:
+                mask = self.torch.zeros(sim.nenv, dtype=self.torch.uint8, device=sim.device)
+                mask[self.torch.as_tensor(idx, device=sim.device)] = 1
+            sim.set_const(mask=mask)
