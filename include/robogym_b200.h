@@ -62,7 +62,9 @@ enum rg_field {
   RG_FIELD_CONTACT = 14,   /* [nenv][contact capacity][4] out (optional): geom1, geom2, dist, condim (rg_batch_capacity) */
   RG_FIELD_NCON = 15,      /* [nenv] int32        out    (optional) */
   RG_FIELD_WARN = 16,      /* [nenv] int32        in/out (optional): bit0 contact buffer full, bit1 row buffer full, bit2 bad state -> reset,
-                              bit3 MPR, bit4 tendon Jacobian too dense, bit5 a contact touched more dofs than the batch allows (dropped) */
+                              bit3 MPR, bit4 tendon Jacobian too dense, bit5 a contact touched more dofs than the batch allows (dropped),
+                              bit6 rg_batch_update_pairs: pair list full (surplus dropped), bit7 rg_batch_update_pairs: a geom_dataid value
+                              that is neither -1 nor a mesh id of a mesh geom (that geom is disabled) */
   RG_FIELD_DBG = 17,       /* [nenv][rg_batch_dbg_size] out (optional): stage dump used by the parity tests */
   RG_FIELD_BODY_XVEL = 18, /* [nenv][nbody*6]     out    (optional): angular, linear velocity of every body frame in world axes
                               = data.get_body_xvelr / get_body_xvelp (robogym/robot/ur16e/mujoco/joint_controlled_arm.py:32,
@@ -78,8 +80,11 @@ enum rg_field {
   RG_NFIELDS = 22
 };
 #define RG_MAX_CONTACTS 32   /* DEFAULT contact capacity of a batch (rg_batch_create); rg_batch_create_ex picks another */
-#define RG_MAX_PARAM_OVERRIDES 16
+#define RG_MAX_PARAM_OVERRIDES 24
 
+/* A mesh geom whose geom_dataid is -1 is a DISABLED part: an empty part slot of a model that holds a different object per
+ * environment (robogym_b200.rearrange_mesh_scene).  It never reaches collision; batches of such a model stream
+ * per-environment pair lists (rg_batch_update_pairs) from the start, derived from the shared geom_dataid row. */
 int rg_model_load(const void* blob, size_t len, int device, rg_model** out);
 void rg_model_destroy(rg_model* m);
 /* value of a dimension of rg_model_fields.h (nq, nv, nu, nbody, ...) or -1 */
@@ -122,8 +127,27 @@ int rg_batch_bind(rg_batch* b, int field, void* device_ptr);
  * device_ptr is a float32 [nenv][count(name)] tensor that replaces the shared array `name` for each environment.
  * Up to RG_MAX_PARAM_OVERRIDES arrays; device_ptr == NULL removes the override.  body_pos rows of bodies attached
  * to the world must be given relative to rg_model_origin().  "mesh_scale" ([nenv][nmesh], see rg_model_set_field) gives every
- * environment its own hull sizes; its values must be finite and > 0 (not checked on the device). */
+ * environment its own hull sizes; its values must be finite and > 0 (not checked on the device).
+ * "geom_dataid" is the one int array: an int32 [nenv][ngeom] row of mesh ids per environment (-1 = disabled part; every
+ * other geom keeps -1), copied bit for bit into the environment's model view.  Binding it gives the batch per-environment
+ * pair lists and marks them all stale: the next step (or rg_batch_update_pairs) derives them from the rows. */
 int rg_batch_bind_param(rg_batch* b, const char* name, void* device_ptr);
+/* Per-environment pair lists (reset time, not per step): one warp per environment whose mask byte is non-zero (mask == NULL:
+ * all) compacts the static candidate pair list, in order, to the pairs whose two geoms are both enabled in that environment's
+ * geom_dataid row, and clears its separating-axis cache.  The collision stage then streams that list instead of the static
+ * one.  A full list sets warning bit 6 (surplus dropped), a bad geom_dataid value bit 7 (the geom counts as disabled).
+ * Fails when geom_dataid is not bound per environment.  Asynchronous on `stream`. */
+int rg_batch_update_pairs(rg_batch* b, const uint8_t* mask_device, void* stream);
+/* The geom_dataid rows of the environments whose mask byte is non-zero (mask == NULL: all) were edited: their lists are stale.
+ * The next rg_step / rg_step_subset / rg_forward first rederives every stale list (the same compaction, on its stream), so a
+ * list never names a part that its row has disabled.  Call it after every write into the bound geom_dataid rows that is not
+ * followed by rg_batch_update_pairs for the same environments (BatchedSim.set_param does).  Asynchronous on `stream`. */
+int rg_batch_mark_pairs_stale(rg_batch* b, const uint8_t* mask_device, void* stream);
+/* capacity of every environment's list (default, or 0: npair).  Set-up call (reallocates, synchronises); the lists are derived
+ * again (from the per-environment rows before the next step, or at once from the shared row); overflow sets warning bit 6. */
+int rg_batch_set_pair_capacity(rg_batch* b, int capacity);
+/* capacity and the device array [nenv] of list lengths (0 / NULL when the batch streams the static list) */
+int rg_batch_pair_info(const rg_batch* b, int* capacity, const int** counts_device);
 int rg_model_origin(const rg_model* m, float origin[3]);
 /* Work-ordered scheduling (default on; RG_BALANCE=0 in the environment turns it off at create): every launch records a
  * per-environment work estimate and the next launch groups environments of similar cost into the same CTA, which

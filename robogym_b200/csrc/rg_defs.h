@@ -156,7 +156,9 @@ enum { RG_DSBL_CONSTRAINT = 1, RG_DSBL_EQUALITY = 2, RG_DSBL_FRICTIONLOSS = 4, R
        RG_DSBL_ACTUATION = 1024, RG_DSBL_REFSAFE = 2048 };
 enum { RG_EL_FLOSS = 0, RG_EL_JLIMIT = 1, RG_EL_TLIMIT = 2 };
 enum { RG_EQ_CONNECT = 0, RG_EQ_WELD = 1, RG_EQ_JOINT = 2 };
-enum { RG_WARN_CONTACT_FULL = 1, RG_WARN_ROWS_FULL = 2, RG_WARN_BAD_STATE = 4, RG_WARN_MPR = 8, RG_WARN_TENDON_NNZ = 16, RG_WARN_DOFS_FULL = 32 };
+enum { RG_WARN_CONTACT_FULL = 1, RG_WARN_ROWS_FULL = 2, RG_WARN_BAD_STATE = 4, RG_WARN_MPR = 8, RG_WARN_TENDON_NNZ = 16, RG_WARN_DOFS_FULL = 32,
+       RG_WARN_PAIRS_FULL = 64 /* rg_batch_update_pairs: the environment's pair list overflowed its capacity (surplus dropped) */,
+       RG_WARN_BAD_DATAID = 128 /* rg_batch_update_pairs: a geom_dataid value that is neither -1 nor a mesh id of a mesh geom (geom disabled) */ };
 
 /* Device view of the compiled model: fp32 / int32 copies of every rg_model_fields.h array. */
 struct RgModel {
@@ -175,7 +177,8 @@ struct RgModel {
   const int* eqrow;            /* [neqrow]: equality id * 8 + row (weld: 6 rows, joint coupling: 1); row k is "virtual tendon" ntendon + k */
   const float* mesh_scale;     /* [nmesh]: uniform scale of every hull (1 at load; model-wide or per-environment parameter) */
   const float* mesh_vert4;     /* [nmeshvert][4]: hull vertices padded to 16 bytes (one vector load each) */
-  const unsigned short* pair_packed; /* [npair] geom1 | geom2 << 8 when ngeom <= 256 (staged in shared memory), else nullptr */
+  const unsigned short* pair_packed; /* [npair] geom1 | geom2 << 8 when ngeom <= 256 (staged in shared memory), else nullptr;
+                                        a view with pair_geom2 == nullptr streams an environment's own list instead (rg_pair) */
   float origin[3];             /* world translation applied at load so coordinates stay small in fp32 */
   int small_bytes;             /* leading part of the arena that is staged into shared memory */
   int nM;                      /* entries of the tree-sparse mass matrix: sum over dofs of (depth + 1) */

@@ -48,6 +48,10 @@ struct RgKernelArgs {
   int* counter;       /* device: next unassigned slot of this launch (zeroed before the launch) */
   int setconst[6];    /* nsub < 0 = an rg_set_const launch: override slots of dof_invweight0, body_invweight0, tendon_invweight0,
                          tendon_length0, body_subtreemass, opt_meaninertia (-1 = not bound per environment, not written) */
+  /* per-environment pair lists (rg_batch_update_pairs) or nullptr = every environment streams the static list */
+  const unsigned* env_pairs;   /* [nenv][pair_cap] g1 | g2 << 16 */
+  const int* env_npair;        /* [nenv] */
+  int pair_cap;
 };
 
 __device__ __forceinline__ uint32_t rg_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -133,7 +137,7 @@ __global__ void __launch_bounds__(RG_MAX_WARPS * 32, 1) rg_step_kernel(const __g
   /* with per-env overrides every warp keeps its own model view + a copy of this env's rows after the scratch */
   RgModelDev* wm = sm;
   float* wover = nullptr;
-  if (args.nover > 0) {
+  if (args.nover > 0 || args.env_pairs) {
     unsigned char* base = (unsigned char*)(scratch0 + (size_t)args.warps * args.L.total) + (size_t)warp * (model_bytes + 4 * args.over_floats);
     wm = (RgModelDev*)base;
     wover = (float*)(base + model_bytes);
@@ -159,15 +163,22 @@ __global__ void __launch_bounds__(RG_MAX_WARPS * 32, 1) rg_step_kernel(const __g
     __syncthreads();
     if (warp >= nact) continue;
     const int e = args.order ? args.order[slot0 + warp] : slot0 + warp;
-    if (args.nover > 0) {
+    if (args.nover > 0 || args.env_pairs) {
       const int lane = threadIdx.x & 31;
       for (int i = lane; i < (int)(sizeof(RgModelDev) / 4); i += 32) ((int*)wm)[i] = ((const int*)sm)[i];
+      /* plain 32-bit loads and stores: the int rows of geom_dataid pass through this float copy bit for bit */
       for (int o = 0; o < args.nover; o++) {
         const float* src = args.over_ptr[o] + (size_t)e * args.over_cnt[o];
         for (int i = lane; i < args.over_cnt[o]; i += 32) wover[args.over_dst[o] + i] = src[i];
       }
       __syncwarp();
       if (lane < args.nover) *(int*)((char*)wm + args.over_off[lane]) = (int)((unsigned char*)(wover + args.over_dst[lane]) - rg_smem_raw);
+      if (args.env_pairs && lane == 0) {   /* stage A streams this environment's own list (rg_pair) */
+        wm->has_pairs = 0;
+        wm->pair_geom1 = (const int*)(args.env_pairs + (size_t)e * args.pair_cap);
+        wm->pair_geom2 = nullptr;
+        wm->npair = args.env_npair[e];
+      }
       __syncwarp();
     }
     if (args.nsub < 0) {
@@ -245,6 +256,24 @@ __global__ void __launch_bounds__(1024) rg_subset_kernel(const uint8_t* __restri
   }
   if (t == 0) *count = base;
 }
+/* rg_batch_update_pairs: one warp per selected environment compacts the static pair list to the pairs whose geoms are both
+   enabled in that environment's geom_dataid row (row stride 0: the shared row), clears its separating-axis cache, whose
+   keys are indices into the list, and its "list is stale" flag.  `mask` may be the stale flags themselves (no __restrict__):
+   every lane reads the environment's byte before lane 0 clears it. */
+__global__ void __launch_bounds__(256) rg_pairs_kernel(RgModel m, const int* __restrict__ dataid, size_t stride, const uint8_t* mask, uint8_t* stale,
+                                                       int nenv, unsigned* __restrict__ pairs, int* __restrict__ npair, int cap, int* __restrict__ sep, int* __restrict__ warn) {
+  const int env = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (env >= nenv || (mask && !mask[env])) return;
+  int w = 0;
+  const int n = rg_env_pairs(m, dataid + (size_t)env * stride, pairs + (size_t)env * cap, cap, &w);
+  for (int i = lane; i < RG_NSEP; i += 32) sep[(size_t)env * RG_NSEP + i] = 0xfff;
+  if (lane == 0) { npair[env] = n; if (warn) warn[env] |= w; if (stale) stale[env] = 0; }
+}
+/* rg_batch_mark_pairs_stale with a mask */
+__global__ void rg_mark_kernel(const uint8_t* __restrict__ mask, uint8_t* __restrict__ stale, int nenv) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e < nenv && mask[e]) stale[e] = 1;
+}
 __global__ void rg_iota_kernel(int* order, int* cost, int* sep, int nenv) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e < nenv) { order[e] = e; cost[e] = 0; for (int i = 0; i < RG_NSEP; i++) sep[(size_t)e * RG_NSEP + i] = 0xfff; }
@@ -259,6 +288,7 @@ struct rg_model {
   RgLayout L;
   std::vector<std::string> names;
   std::vector<size_t> src_counts;
+  bool disabled_parts = false;   /* some mesh geom has geom_dataid -1: its batches always stream per-environment pair lists */
 };
 struct rg_batch {
   const rg_model* model;
@@ -278,6 +308,11 @@ struct rg_batch {
   int* d_sep = nullptr;    /* [nenv][RG_NSEP] separating-axis cache of the narrow phase (speeds it up; results do not depend on it) */
   int balance = 1;
   int groups = 1;          /* barrier groups per round (rg_batch_set_barrier_groups) */
+  unsigned* d_pairs = nullptr;  /* [nenv][pair_cap] per-environment pair lists (rg_batch_update_pairs), or nullptr */
+  int* d_npair = nullptr;       /* [nenv] their lengths */
+  int pair_cap = 0;
+  uint8_t* d_stale = nullptr;   /* [nenv] the environment's geom_dataid row may have changed since its list was derived */
+  bool any_stale = false;       /* some d_stale byte may be set: the next step rederives those lists first */
 };
 
 static void rg_wire_device_view(rg_model* mm) {
@@ -313,6 +348,15 @@ int rg_model_load(const void* blob, size_t len, int device, rg_model** out) {
   std::string err;
   if (!rg_host_load(blob, len, mm->hm, err)) { delete mm; return rg_fail(-1, "rg_model_load: " + err); }
   mm->device = device;
+  {
+    const RgModel& v = mm->hm.view;
+    for (int g = 0; g < v.ngeom; g++) {
+      if (v.geom_type[g] != RG_GEOM_MESH) continue;
+      if (v.geom_dataid[g] < -1 || v.geom_dataid[g] >= v.nmesh) { delete mm; return rg_fail(-1, "rg_model_load: geom_dataid of a mesh geom is neither -1 nor a mesh id"); }
+      if (v.geom_dataid[g] == -1) mm->disabled_parts = true;
+    }
+    if (mm->disabled_parts && v.ngeom > 65536) { delete mm; return rg_fail(-1, "rg_model_load: disabled mesh parts need ngeom <= 65536 (16-bit ids in the pair lists)"); }
+  }
   mm->L = rg_make_layout(mm->hm.view);
   cudaError_t e = cudaSetDevice(device);
   if (e == cudaSuccess) e = cudaMalloc((void**)&mm->d_arena, mm->hm.arena.size());
@@ -411,7 +455,9 @@ int rg_model_set_field_async(rg_model* mm, const char* name, const void* data, s
     float* aabb = (float*)m.geom_aabb;
     for (int g = 0; g < m.ngeom; g++) {
       if (m.geom_type[g] != RG_GEOM_MESH) continue;
-      const int mid = m.geom_dataid[g], a = m.mesh_vertadr[mid], nvt = m.mesh_vertnum[mid];
+      const int mid = m.geom_dataid[g];
+      if (mid < 0) continue;   /* a disabled part */
+      const int a = m.mesh_vertadr[mid], nvt = m.mesh_vertnum[mid];
       for (int k = 0; k < 3 && nvt > 0; k++) {
         double lo = v[3 * a + k], hi = lo;
         for (int q = 1; q < nvt; q++) { lo = fmin(lo, v[3 * (a + q) + k]); hi = fmax(hi, v[3 * (a + q) + k]); }
@@ -442,7 +488,7 @@ static int rg_batch_size(rg_batch* b) {
   const int model_bytes = RG_MODEL_DEV_BYTES;
   const int fixed = model_bytes + (int)((m->hm.small_bytes + 127) & ~(size_t)127) + 64;
   /* with per-env parameter overrides every warp also holds its own model view + this env's rows */
-  const int per_warp = 4 * b->L.total + (b->nover > 0 ? model_bytes + 4 * b->over_floats : 0);
+  const int per_warp = 4 * b->L.total + (b->nover > 0 || b->d_pairs ? model_bytes + 4 * b->over_floats : 0);
   int warps = (maxsmem - fixed) / per_warp;
   if (warps < 1) return rg_fail(-3, "rg_batch: model scratch does not fit in shared memory");
   if (warps > RG_MAX_WARPS) warps = RG_MAX_WARPS;
@@ -467,6 +513,37 @@ static int rg_batch_size(rg_batch* b) {
   return 0;
 }
 
+/* (re)allocate the per-environment pair lists with `cap` entries each (set-up call: synchronises) */
+static int rg_pairs_alloc(rg_batch* b, int cap) {
+  RG_CUDA(cudaSetDevice(b->model->device));
+  if (b->d_pairs) { RG_CUDA(cudaFree(b->d_pairs)); b->d_pairs = nullptr; }
+  if (!b->d_npair) RG_CUDA(cudaMalloc((void**)&b->d_npair, sizeof(int) * (size_t)b->nenv));
+  if (!b->d_stale) { RG_CUDA(cudaMalloc((void**)&b->d_stale, (size_t)b->nenv)); RG_CUDA(cudaMemset(b->d_stale, 0, (size_t)b->nenv)); }
+  b->pair_cap = cap > 0 ? cap : (b->model->hm.view.npair > 0 ? b->model->hm.view.npair : 1);
+  RG_CUDA(cudaMalloc((void**)&b->d_pairs, sizeof(unsigned) * (size_t)b->nenv * b->pair_cap));
+  return 0;
+}
+/* every environment's list from the shared geom_dataid row (a model with disabled parts, no per-environment row bound) */
+static int rg_pairs_from_shared(rg_batch* b) {
+  const rg_model* m = b->model;
+  rg_pairs_kernel<<<(b->nenv + 7) / 8, 256>>>(m->dev, m->dev.geom_dataid, 0, nullptr, b->d_stale, b->nenv, b->d_pairs, b->d_npair, b->pair_cap, b->d_sep,
+                                              (int*)b->ptr[RG_FIELD_WARN]);
+  RG_CUDA(cudaGetLastError());
+  RG_CUDA(cudaDeviceSynchronize());
+  b->any_stale = false;
+  return 0;
+}
+/* every list stale: derived from the per-environment rows before the next step (set-up call: synchronises) */
+static int rg_pairs_all_stale(rg_batch* b) {
+  RG_CUDA(cudaMemset(b->d_stale, 1, (size_t)b->nenv));
+  b->any_stale = true;
+  return 0;
+}
+static int rg_find_override(const rg_batch* b, const char* name) {
+  for (int i = 0; i < b->nover; i++) if (b->over_name[i] == name) return i;
+  return -1;
+}
+
 int rg_batch_create(const rg_model* m, int nenv, rg_batch** out) { return rg_batch_create_ex(m, nenv, 0, 0, 0, out); }
 
 int rg_batch_create_ex(const rg_model* m, int nenv, int contact_capacity, int row_capacity, int dofs_per_contact, rg_batch** out) {
@@ -489,6 +566,12 @@ int rg_batch_create_ex(const rg_model* m, int nenv, int contact_capacity, int ro
   if (e == cudaSuccess) e = cudaMalloc((void**)&b->d_sep, sizeof(int) * (size_t)nenv * RG_NSEP);
   if (e == cudaSuccess) { rg_iota_kernel<<<(nenv + 255) / 256, 256>>>(b->d_order, b->d_cost, b->d_sep, nenv); e = cudaDeviceSynchronize(); }   /* set-up call: may synchronise (the stepping calls never do) */
   if (e != cudaSuccess) { std::string msg = std::string("rg_batch_create: CUDA: ") + cudaGetErrorString(e); rg_batch_destroy(b); return rg_fail(-2, msg); }
+  if (m->disabled_parts) {   /* the static list holds disabled parts: stream the shared draw's own pairs from the start */
+    int rc2 = rg_pairs_alloc(b, 0);
+    if (!rc2) rc2 = rg_batch_size(b);
+    if (!rc2) rc2 = rg_pairs_from_shared(b);
+    if (rc2) { const std::string msg = g_err; rg_batch_destroy(b); return rg_fail(rc2, msg); }
+  }
   *out = b;
   return 0;
 }
@@ -499,6 +582,9 @@ void rg_batch_destroy(rg_batch* b) {
   if (b->d_subset) cudaFree(b->d_subset);
   if (b->d_sep) cudaFree(b->d_sep);
   if (b->d_counter) cudaFree(b->d_counter);
+  if (b->d_pairs) cudaFree(b->d_pairs);
+  if (b->d_npair) cudaFree(b->d_npair);
+  if (b->d_stale) cudaFree(b->d_stale);
   delete b;
 }
 
@@ -542,7 +628,10 @@ int rg_batch_bind_param(rg_batch* b, const char* name, void* p) {
 #undef RG_IB
 #undef RG_FB
   if (!strcmp(name, "mesh_scale")) { off = (int)offsetof(RgModelDev, mesh_scale); cnt = m.nmesh; }
+  const bool dataid = !strcmp(name, "geom_dataid");   /* the one int array: per-environment mesh draws (rg_batch_update_pairs) */
+  if (dataid) { off = (int)offsetof(RgModelDev, geom_dataid); cnt = ngeom; }
   if (off < 0) return rg_fail(-1, std::string("rg_batch_bind_param: not a (small) float model array: ") + name);
+  if (dataid && ngeom > 65536) return rg_fail(-1, "rg_batch_bind_param: geom_dataid per environment needs ngeom <= 65536 (16-bit ids in the pair lists)");
   int slot = -1;
   for (int i = 0; i < b->nover; i++) if (b->over_name[i] == name) slot = i;
   if (!p) {
@@ -556,7 +645,66 @@ int rg_batch_bind_param(rg_batch* b, const char* name, void* p) {
   int fl = 0;
   for (int i = 0; i < b->nover; i++) { b->over_dst[i] = fl; fl += (b->over_cnt[i] + 3) & ~3; }
   b->over_floats = fl;
-  return rg_batch_size(b);
+  if (dataid && p) {
+    /* the rows are the caller's to fill: every list is rederived from them before the next step (or by rg_batch_update_pairs) */
+    if (!b->d_pairs) { const int rc = rg_pairs_alloc(b, 0); if (rc) return rc; }
+    const int rc = rg_pairs_all_stale(b);
+    if (rc) return rc;
+  }
+  const int rc = rg_batch_size(b);
+  if (rc || !dataid || p) return rc;
+  if (!b->model->disabled_parts) {   /* back to the static list */
+    if (b->d_pairs) { cudaFree(b->d_pairs); b->d_pairs = nullptr; }
+    b->any_stale = false;
+    return rg_batch_size(b);
+  }
+  return rg_pairs_from_shared(b);
+}
+
+int rg_batch_set_pair_capacity(rg_batch* b, int capacity) {
+  if (!b || capacity < 0) return rg_fail(-1, "rg_batch_set_pair_capacity: bad argument");
+  if (!b->d_pairs) return rg_fail(-1, "rg_batch_set_pair_capacity: the batch has no per-environment pair lists (bind geom_dataid first)");
+  int rc = rg_pairs_alloc(b, capacity);
+  if (rc) return rc;
+  if (rg_find_override(b, "geom_dataid") >= 0) return rg_pairs_all_stale(b);
+  return rg_pairs_from_shared(b);
+}
+
+int rg_batch_mark_pairs_stale(rg_batch* b, const uint8_t* mask, void* stream) {
+  if (!b) return rg_fail(-1, "rg_batch_mark_pairs_stale: null argument");
+  if (rg_find_override(b, "geom_dataid") < 0 || !b->d_pairs) return rg_fail(-1, "rg_batch_mark_pairs_stale: geom_dataid is not bound per environment (rg_batch_bind_param)");
+  RG_CUDA(cudaSetDevice(b->model->device));
+  if (mask) rg_mark_kernel<<<(b->nenv + 255) / 256, 256, 0, (cudaStream_t)stream>>>(mask, b->d_stale, b->nenv);
+  else RG_CUDA(cudaMemsetAsync(b->d_stale, 1, (size_t)b->nenv, (cudaStream_t)stream));
+  RG_CUDA(cudaGetLastError());
+  b->any_stale = true;
+  return 0;
+}
+
+/* rederive the lists of the environments selected by `mask` (NULL: all) from the bound geom_dataid rows, on `stream` */
+static int rg_pairs_launch(rg_batch* b, const uint8_t* mask, void* stream) {
+  const int slot = rg_find_override(b, "geom_dataid");
+  if (slot < 0 || !b->d_pairs) return rg_fail(-1, "rg_batch_update_pairs: geom_dataid is not bound per environment (rg_batch_bind_param)");
+  const rg_model* m = b->model;
+  RG_CUDA(cudaSetDevice(m->device));
+  rg_pairs_kernel<<<(b->nenv + 7) / 8, 256, 0, (cudaStream_t)stream>>>(m->dev, (const int*)b->over_ptr[slot], (size_t)m->hm.view.ngeom, mask, b->d_stale, b->nenv,
+                                                                       b->d_pairs, b->d_npair, b->pair_cap, b->d_sep, (int*)b->ptr[RG_FIELD_WARN]);
+  RG_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rg_batch_update_pairs(rg_batch* b, const uint8_t* mask, void* stream) {
+  if (!b) return rg_fail(-1, "rg_batch_update_pairs: null argument");
+  const int rc = rg_pairs_launch(b, mask, stream);
+  if (!rc && !mask) b->any_stale = false;
+  return rc;
+}
+
+int rg_batch_pair_info(const rg_batch* b, int* capacity, const int** counts_device) {
+  if (!b) return rg_fail(-1, "rg_batch_pair_info: null argument");
+  if (capacity) *capacity = b->d_pairs ? b->pair_cap : 0;
+  if (counts_device) *counts_device = b->d_pairs ? b->d_npair : nullptr;
+  return 0;
 }
 
 int rg_batch_capacity(const rg_batch* b, int* contacts, int* rows, int* dofs_per_contact) {
@@ -613,6 +761,12 @@ static int rg_launch_step(rg_batch* b, const uint8_t* mask, int nsub, int final_
   }
   const int rc = rg_fill_io(b, args.io);
   if (rc) return rc;
+  if (b->any_stale && !setconst) {   /* geom_dataid rows written since their lists were derived: those lists first */
+    const int rc2 = rg_pairs_launch(b, b->d_stale, stream);
+    if (rc2) return rc2;
+    b->any_stale = false;
+  }
+  args.env_pairs = b->d_pairs; args.env_npair = b->d_npair; args.pair_cap = b->pair_cap;
   args.m = b->model->dev;
   args.L = b->L;
   args.arena = b->model->d_arena;

@@ -69,6 +69,10 @@ def lib():
         L.rg_forward.argtypes = [vp, vp]
         L.rg_reset.argtypes = [vp, vp, vp]
         L.rg_set_const.argtypes = [vp, vp, vp]
+        L.rg_batch_update_pairs.argtypes = [vp, vp, vp]
+        L.rg_batch_mark_pairs_stale.argtypes = [vp, vp, vp]
+        L.rg_batch_set_pair_capacity.argtypes = [vp, ci]
+        L.rg_batch_pair_info.argtypes = [vp, ctypes.POINTER(ci), ctypes.POINTER(vp)]
         _lib = L
     return _lib
 
@@ -76,6 +80,15 @@ def lib():
 def _check(rc):
     if rc != 0:
         raise EngineError(lib().rg_last_error().decode())
+
+
+def check_geom_dataid(v, m):
+    """Per-environment geom_dataid rows ([rows, ngeom]) must hold -1 or a mesh id on mesh geoms and -1 on every other geom."""
+    a = np.asarray(v.detach().cpu() if hasattr(v, "detach") else v).reshape(-1, m["ngeom"])
+    mesh = np.asarray(m["geom_type"]) == 7
+    ok = np.where(mesh[None, :], (a >= -1) & (a < m["nmesh"]), a == -1)
+    if not ok.all():
+        raise ValueError("geom_dataid: -1 or a mesh id on mesh geoms, -1 on every other geom")
 
 
 def check_mesh_scale(v):
@@ -238,13 +251,26 @@ class BatchedSim:
         """Per-environment override of a float model array (domain randomisation): `values` is [nenv, count]
         (float64/float32 host array or tensor), or [len(idx), count] for the rows `idx` of an array that is already bound.
         The device copy is created on first use and updated in place; rows in world coordinates get the engine's fp32 world
-        shift on EVERY write."""
+        shift on EVERY write.  `geom_dataid` (per-environment mesh draws) is the one int array: it is kept as int32, and the
+        pair lists of the rows written are marked stale, so the next step rederives them unless update_pairs() does first."""
         t = self.torch
         m = self.model.host
         rows = self.nenv if idx is None else len(idx)
+        if name == "geom_dataid":
+            v = t.as_tensor(np.asarray(values) if not t.is_tensor(values) else values).to(t.int64).reshape(rows, -1)
+            if v.shape[1] != m["ngeom"]:
+                raise EngineError(f"set_param(geom_dataid): expected {m['ngeom']} values per environment, got {v.shape[1]}")
+            check_geom_dataid(v, m)
+            out = self._store_param(name, v.to(device=self.device, dtype=t.int32).contiguous(), idx)
+            mp = None
+            if idx is not None:
+                mk = t.zeros(self.nenv, dtype=t.uint8, device=self.device)
+                mk[t.as_tensor(idx, device=self.device).long()] = 1
+                self._keep_stale = mk            # alive until the launch has consumed it
+                mp = ctypes.c_void_p(mk.data_ptr())
+            _check(lib().rg_batch_mark_pairs_stale(self.h, mp, self._stream()))
+            return out
         v = t.as_tensor(np.asarray(values, dtype=np.float64) if not t.is_tensor(values) else values).to(t.float64).reshape(rows, -1).clone()
-        if idx is not None and name not in getattr(self, "_params", {}):
-            raise EngineError(f"set_param({name}, idx=...): bind the full array first")
         count = m["nmesh"] if name == "mesh_scale" else m[name].size     # mesh_scale: the engine's per-hull scale, not a blob array
         if v.shape[1] != count:
             raise EngineError(f"set_param({name}): expected {count} values per environment, got {v.shape[1]}")
@@ -255,7 +281,11 @@ class BatchedSim:
             o = (ctypes.c_float * 3)()
             _check(lib().rg_model_origin(self.model.h, o))
             world_shift_rows(t, v, name, m, list(o))
-        dev = v.to(device=self.device, dtype=t.float32).contiguous()
+        return self._store_param(name, v.to(device=self.device, dtype=t.float32).contiguous(), idx)
+
+    def _store_param(self, name, dev, idx):
+        if idx is not None and name not in getattr(self, "_params", {}):
+            raise EngineError(f"set_param({name}, idx=...): bind the full array first")
         if not hasattr(self, "_params"):
             self._params = {}
         if idx is not None:
@@ -266,6 +296,30 @@ class BatchedSim:
             self._params[name] = dev
             _check(lib().rg_batch_bind_param(self.h, name.encode(), ctypes.c_void_p(dev.data_ptr())))
         return self._params[name]
+
+    def update_pairs(self, mask=None):
+        """Rederive the per-environment pair lists from the bound geom_dataid rows (all environments, or those of `mask`):
+        each keeps the static candidate pairs whose two geoms are enabled in its row (include/robogym_b200.h)."""
+        mp = None
+        if mask is not None:
+            mask = mask.to(device=self.device, dtype=self.torch.uint8).contiguous()
+            mp = ctypes.c_void_p(mask.data_ptr())
+            self._keep_mask = mask
+        _check(lib().rg_batch_update_pairs(self.h, mp, self._stream()))
+
+    def set_pair_capacity(self, capacity):
+        """Pairs each environment's list can hold (0: npair); the lists are derived again before the next step."""
+        _check(lib().rg_batch_set_pair_capacity(self.h, int(capacity)))
+
+    def pair_counts(self):
+        """Length of every environment's pair list ([nenv] int32 device tensor, a copy), or None when the batch streams the
+        static list."""
+        cap, ptr = ctypes.c_int(), ctypes.c_void_p()
+        _check(lib().rg_batch_pair_info(self.h, ctypes.byref(cap), ctypes.byref(ptr)))
+        if not ptr.value:
+            return None
+        view = type("EngineInts", (), {"__cuda_array_interface__": dict(shape=(self.nenv,), typestr="<i4", data=(ptr.value, False), version=2)})()
+        return self.torch.as_tensor(view, device=self.device).clone()
 
     def enable_per_env_timestep(self):
         self.timestep = self.torch.full((self.nenv,), float(self.model.host["opt_timestep"][0]), dtype=self.torch.float32, device=self.device)
