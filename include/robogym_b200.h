@@ -128,6 +128,10 @@ int rg_batch_bind(rg_batch* b, int field, void* device_ptr);
  * Up to RG_MAX_PARAM_OVERRIDES arrays; device_ptr == NULL removes the override.  body_pos rows of bodies attached
  * to the world must be given relative to rg_model_origin().  "mesh_scale" ([nenv][nmesh], see rg_model_set_field) gives every
  * environment its own hull sizes; its values must be finite and > 0 (not checked on the device).
+ * "geom_mesh_scale" ([nenv][ngeom], finite and > 0, not checked on the device) scales every mesh geom of an environment on
+ * top of its hull's mesh_scale: the narrow phase uses the hull scaled by mesh_scale[dataid] * geom_mesh_scale[g], and the OBB
+ * cull scales the geom's geom_aabb by the same product.  Two geoms that share a hull can so have different sizes.  It exists
+ * per environment only (rg_model_set_field refuses it); while it is not bound every factor is 1.
  * "geom_dataid" is the one int array: an int32 [nenv][ngeom] row of mesh ids per environment (-1 = disabled part; every
  * other geom keeps -1), copied bit for bit into the environment's model view.  Binding it gives the batch per-environment
  * pair lists and marks them all stale: the next step (or rg_batch_update_pairs) derives them from the rows. */

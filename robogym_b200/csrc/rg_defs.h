@@ -176,6 +176,8 @@ struct RgModel {
   const int* dof_sidx;         /* [2 nv]: solver position of every dof (or -1), then the dof at every solver position */
   const int* eqrow;            /* [neqrow]: equality id * 8 + row (weld: 6 rows, joint coupling: 1); row k is "virtual tendon" ntendon + k */
   const float* mesh_scale;     /* [nmesh]: uniform scale of every hull (1 at load; model-wide or per-environment parameter) */
+  const float* geom_mesh_scale; /* [ngeom]: uniform scale of every mesh geom on top of its hull's mesh_scale (per-environment
+                                   parameter only), or nullptr = 1 everywhere */
   const float* mesh_vert4;     /* [nmeshvert][4]: hull vertices padded to 16 bytes (one vector load each) */
   const unsigned short* pair_packed; /* [npair] geom1 | geom2 << 8 when ngeom <= 256 (staged in shared memory), else nullptr;
                                         a view with pair_geom2 == nullptr streams an environment's own list instead (rg_pair) */
@@ -235,6 +237,7 @@ struct RgModelDev {
   RgArr<int> dof_sidx;
   RgArr<int> eqrow;
   RgArr<float> mesh_scale;
+  RgArr<float> geom_mesh_scale;   /* off < 0 while no per-environment row is bound: never staged, so it costs no shared memory */
   RgArr<unsigned short> pair_packed;
   int has_pairs;
   const float* mesh_vert4;
@@ -249,6 +252,7 @@ struct RgModelDev {
 };
 #define RG_MODEL_T RgModelDev
 #define RG_HAS_PAIRS(m) ((m).has_pairs)
+#define RG_GEOM_MESH_SCALE(m, g) ((m).geom_mesh_scale.off >= 0 ? (m).geom_mesh_scale[g] : 1.0f)
 /* the model view is handed to non-inlined code as its byte offset in the CTA's dynamic shared memory, so that
    every access through it compiles to LDS rather than a generic load */
 typedef int RgMRef;
@@ -257,6 +261,7 @@ typedef int RgMRef;
 #else
 #define RG_MODEL_T RgModel
 #define RG_HAS_PAIRS(m) ((m).pair_packed != nullptr)
+#define RG_GEOM_MESH_SCALE(m, g) ((m).geom_mesh_scale ? (m).geom_mesh_scale[g] : 1.0f)
 typedef const RgModel* RgMRef;
 #define RG_MDEREF(r) (*(r))
 #define RG_MREF(m) (&(m))

@@ -57,6 +57,8 @@ struct RgKernelArgs {
 __device__ __forceinline__ uint32_t rg_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 #define RG_MODEL_DEV_BYTES ((int)((sizeof(RgModelDev) + 127) & ~(size_t)127))
+/* every warp with overrides keeps its own copy of the view: 128 B more would cost dactyl/locked a resident environment per SM */
+static_assert(sizeof(RgModelDev) <= 1024, "the device model view must fit in 1024 bytes of shared memory");
 
 __global__ void __launch_bounds__(RG_MAX_WARPS * 32, 1) rg_step_kernel(const __grid_constant__ RgKernelArgs args) {
   unsigned char* smem_raw = rg_smem_raw;
@@ -109,6 +111,7 @@ __global__ void __launch_bounds__(RG_MAX_WARPS * 32, 1) rg_step_kernel(const __g
     RG_SETPTR(mesh_vert4)
     if (lane == 0) {
       sm->has_pairs = args.m.pair_packed != nullptr;
+      sm->geom_mesh_scale.off = -1;   /* unbound: every factor 1 (a bound row overwrites the offset in the warp's own view) */
       sm->pair_packed.off = args.m.pair_packed ? model_bytes + (int)((const char*)args.m.pair_packed - abase) : 0;
       sm->origin[0] = args.m.origin[0]; sm->origin[1] = args.m.origin[1]; sm->origin[2] = args.m.origin[2];
       sm->small_bytes = small_bytes;
@@ -422,6 +425,8 @@ int rg_model_set_field_async(rg_model* mm, const char* name, const void* data, s
 #undef RG_DIM
 #undef RG_I
 #undef RG_F
+  if (!strcmp(name, "geom_mesh_scale"))
+    return rg_fail(-1, "rg_model_set_field: geom_mesh_scale exists per environment only (rg_batch_bind_param); scale hulls model-wide with mesh_scale");
   const bool is_scale = !strcmp(name, "mesh_scale");   /* derived array of the engine, not a blob field */
   if (is_scale) { hptr = (void*)m.mesh_scale; n = (size_t)m.nmesh; }
   if (!hptr) return rg_fail(-1, std::string("rg_model_set_field: unknown field ") + name);
@@ -628,6 +633,7 @@ int rg_batch_bind_param(rg_batch* b, const char* name, void* p) {
 #undef RG_IB
 #undef RG_FB
   if (!strcmp(name, "mesh_scale")) { off = (int)offsetof(RgModelDev, mesh_scale); cnt = m.nmesh; }
+  if (!strcmp(name, "geom_mesh_scale")) { off = (int)offsetof(RgModelDev, geom_mesh_scale); cnt = ngeom; }
   const bool dataid = !strcmp(name, "geom_dataid");   /* the one int array: per-environment mesh draws (rg_batch_update_pairs) */
   if (dataid) { off = (int)offsetof(RgModelDev, geom_dataid); cnt = ngeom; }
   if (off < 0) return rg_fail(-1, std::string("rg_batch_bind_param: not a (small) float model array: ") + name);

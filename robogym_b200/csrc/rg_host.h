@@ -245,6 +245,7 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
   float* mscale = (float*)(base + off_mscale);
   for (int k = 0; k < m.nmesh; k++) mscale[k] = 1.0f;
   m.mesh_scale = mscale;
+  m.geom_mesh_scale = nullptr;   /* per-environment only (rg_batch_bind_param): never part of the arena */
   hm.offsets.push_back(off_mscale);
   /* hull vertices padded to float4: the narrow phase scans a hull's vertices with one 16-byte load each */
   float* v4 = (float*)(base + off_v4);

@@ -91,12 +91,12 @@ def check_geom_dataid(v, m):
         raise ValueError("geom_dataid: -1 or a mesh id on mesh geoms, -1 on every other geom")
 
 
-def check_mesh_scale(v):
-    """mesh_scale values must be finite and > 0: the narrow phase scales the arg-max vertex of the unscaled hull, which is
-    the scaled hull's support point only for a positive scale."""
+def check_mesh_scale(v, name="mesh_scale"):
+    """mesh_scale (and geom_mesh_scale) values must be finite and > 0: the narrow phase scales the arg-max vertex of the
+    unscaled hull, which is the scaled hull's support point only for a positive scale."""
     a = np.asarray(v.detach().cpu() if hasattr(v, "detach") else v, dtype=np.float64)
     if not (np.isfinite(a).all() and (a > 0).all()):
-        raise ValueError("mesh_scale must be finite and positive")
+        raise ValueError(f"{name} must be finite and positive")
 
 
 class DeviceModel:
@@ -117,7 +117,10 @@ class DeviceModel:
     def set_field(self, name, values, stream=None):
         """Overwrite a model array (randomisers write e.g. geom_friction, dof_damping, opt_gravity).  The upload is ordered
         on `stream` (a raw cudaStream_t; default: torch's current stream on the model's device when torch is loaded).
-        `mesh_scale` ([nmesh], finite and > 0) scales every hull uniformly without touching mesh_vert."""
+        `mesh_scale` ([nmesh], finite and > 0) scales every hull uniformly without touching mesh_vert.  `geom_mesh_scale` exists
+        per environment only (BatchedSim.set_param)."""
+        if name == "geom_mesh_scale":
+            raise ValueError("geom_mesh_scale is a per-environment array (BatchedSim.set_param); scale hulls model-wide with mesh_scale")
         if name == "mesh_scale":
             check_mesh_scale(values)
         arr = self.mesh_scale if name == "mesh_scale" else self.host[name]
@@ -252,7 +255,9 @@ class BatchedSim:
         (float64/float32 host array or tensor), or [len(idx), count] for the rows `idx` of an array that is already bound.
         The device copy is created on first use and updated in place; rows in world coordinates get the engine's fp32 world
         shift on EVERY write.  `geom_dataid` (per-environment mesh draws) is the one int array: it is kept as int32, and the
-        pair lists of the rows written are marked stale, so the next step rederives them unless update_pairs() does first."""
+        pair lists of the rows written are marked stale, so the next step rederives them unless update_pairs() does first.
+        Besides the blob's arrays: `mesh_scale` ([nmesh]) and `geom_mesh_scale` ([ngeom], a mesh geom's own scale on top of
+        its hull's; finite and > 0, 1 while unbound), the engine's uniform hull scales."""
         t = self.torch
         m = self.model.host
         rows = self.nenv if idx is None else len(idx)
@@ -271,11 +276,12 @@ class BatchedSim:
             _check(lib().rg_batch_mark_pairs_stale(self.h, mp, self._stream()))
             return out
         v = t.as_tensor(np.asarray(values, dtype=np.float64) if not t.is_tensor(values) else values).to(t.float64).reshape(rows, -1).clone()
-        count = m["nmesh"] if name == "mesh_scale" else m[name].size     # mesh_scale: the engine's per-hull scale, not a blob array
+        # mesh_scale / geom_mesh_scale: the engine's per-hull / per-mesh-geom scales, not blob arrays
+        count = {"mesh_scale": m["nmesh"], "geom_mesh_scale": m["ngeom"]}[name] if name in ("mesh_scale", "geom_mesh_scale") else m[name].size
         if v.shape[1] != count:
             raise EngineError(f"set_param({name}): expected {count} values per environment, got {v.shape[1]}")
-        if name == "mesh_scale":
-            check_mesh_scale(v)
+        if name in ("mesh_scale", "geom_mesh_scale"):
+            check_mesh_scale(v, name)
         if name in ("body_pos", "geom_pos", "site_pos"):
             # keep the engine's fp32 world shift: bodies attached to the world, and geoms / sites attached to the world body
             o = (ctypes.c_float * 3)()

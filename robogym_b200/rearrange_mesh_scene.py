@@ -11,8 +11,17 @@ the parts that exist.
 * `ObjectLibrary.from_blobs(*blobs)`: the objects of compiled rearrange scenes (hulls, part geom rows, body rows), identical
   ones merged.
 * `slotted_model(base, library)`: the padded model every environment of a batch shares.
-* `compact_model(base, library, draw)`: the model the reference would build for one draw (exactly the parts drawn).
-* `BatchedMeshScene(sim, library)`: writes a draw per environment into a batch of the slotted model.
+* `compact_model(base, library, draw, scale)`: the model the reference would build for one draw (exactly the parts drawn), with
+  every object at its own scale.
+* `BatchedMeshScene(sim, library)`: writes a draw per environment into a batch of the slotted model, each object at its own
+  scale.
+
+Object scale.  The reference compiles every object with `<mesh scale="s s s">` on each of its parts (common/utils.py:250-281,
+make_mesh_object; s from common/mesh.py:66-102 and simulation/mesh.py:59, restated by `ObjectLibrary.object_scales`).  The
+compiler then scales the hull, the part's position in its body, its size, bounding sphere and bounding box by s, the body's mass
+by s^3, its inertia by s^5 and its centre of mass by s (`SCALED_PART_FIELDS`, `scaled_body_rows`).  Two slots that draw the same
+object share its library hulls, so a batch scales a part in the narrow phase with the engine's per-environment
+`geom_mesh_scale` row instead of editing the hull; its geom_aabb stays the unscaled hull's, which the engine scales.
 """
 import numpy as np
 
@@ -27,6 +36,8 @@ BODY_FIELDS = ("body_mass", "body_inertia", "body_ipos", "body_iquat")
 SCENE_GEOM_FIELDS = ("geom_pos", "geom_quat", "geom_size", "geom_rbound", "geom_aabb")
 GEOM_ARRAYS = [name for _, name, cnt in modelblob.ARRAYS if cnt.split("*")[0].strip() == "ngeom"]
 SET_CONST_FIELDS = ("dof_invweight0", "body_invweight0", "body_subtreemass", "opt_meaninertia")
+# part rows that scale with the object (geom_aabb too in a compiled model, but not in a batch: the engine scales it there)
+SCALED_PART_FIELDS = ("geom_pos", "geom_size", "geom_rbound")
 # part rows a draw does NOT write per environment: the int ones cannot be bound per environment, and the material ones are
 # set per slot (BatchedMeshScene.set_material), not per object.  Every part of every library object must share them.
 SHARED_PART_FIELDS = tuple(f for f in PART_FIELDS if f not in SCENE_GEOM_FIELDS)
@@ -34,6 +45,12 @@ SHARED_PART_FIELDS = tuple(f for f in PART_FIELDS if f not in SCENE_GEOM_FIELDS)
 
 def _rows(m, name, count_name):
     return np.asarray(m[name]).reshape(m[count_name], -1)
+
+
+def scaled_body_rows(body, s):
+    """an object's body rows (BODY_FIELDS) at uniform scale s: mass s^3, inertia s^5, centre of mass s, principal axes kept"""
+    return dict(body_mass=body["body_mass"] * s ** 3, body_inertia=body["body_inertia"] * s ** 5, body_ipos=body["body_ipos"] * s,
+                body_iquat=body["body_iquat"])
 
 
 def _slot_bodies(m, names):
@@ -68,13 +85,24 @@ class LibraryEntry:
         self.key = b"".join([h.key for h in hulls] + [np.ascontiguousarray(parts[f]).tobytes() for f in PART_FIELDS]
                             + [np.ascontiguousarray(body[f]).tobytes() for f in BODY_FIELDS])
 
+    def _points(self):
+        """every hull vertex in the body frame"""
+        return np.concatenate([h.vert @ _quat2mat(self.parts["geom_quat"][j]).T + self.parts["geom_pos"][j] for j, h in enumerate(self.hulls)])
+
     def lowest_point(self):
-        """lowest hull point of the object in its body frame (z), for placing it on a surface"""
+        """lowest hull point of the object in its body frame (z), for placing it on a surface (at scale s: s times this)"""
         z = np.inf
         for j, h in enumerate(self.hulls):
             R = _quat2mat(self.parts["geom_quat"][j])
             z = min(z, float((h.vert @ R.T)[:, 2].min() + self.parts["geom_pos"][j][2]))
         return z
+
+    @property
+    def extents(self):
+        """[3] size of the object's axis-aligned box in its body frame.  A hull keeps the extreme points of its mesh, so this is
+        what the reference measures as get_combined_mesh(files).extents (common/mesh.py:76-80)."""
+        p = self._points()
+        return p.max(0) - p.min(0)
 
 
 def _quat2mat(q):
@@ -124,10 +152,37 @@ class ObjectLibrary:
     def max_parts(self):
         return max(self.part_counts)
 
+    def object_scales(self, draw, size_scale, mesh_scale=1.0, normalize_mesh=False, normalized_mesh_size=0.05):
+        """The scale the reference compiles each drawn object with ([nenv, nslot] float64; 1 for an empty slot), from the
+        randomised size scales `size_scale` [nenv, nslot] (sample_object_size_scales), as MeshRearrangeEnv._recreate_sim
+        (common/mesh.py:66-102) and make_objects_xml (simulation/mesh.py:59) compute it: in an environment with 10 or more
+        objects (drawn slots; the reference's num_objects) no object is scaled up by its size scale and all shrink by
+        (10 / n) ** 0.5; `normalize_mesh` scales an object so that half its largest extent is `normalized_mesh_size`;
+        `mesh_scale` (simulation_params.mesh_scale) multiplies everything."""
+        draw = np.asarray(draw.cpu() if hasattr(draw, "cpu") else draw, dtype=np.int64)
+        size = np.broadcast_to(np.asarray(size_scale.cpu() if hasattr(size_scale, "cpu") else size_scale, dtype=np.float64), draw.shape)
+        n = (draw >= 0).sum(-1, keepdims=True)
+        glob = np.where(n < 10, 1.0, np.sqrt(10.0 / np.maximum(n, 1)))
+        s = np.where(n >= 10, np.minimum(size, 1.0), size)
+        if normalize_mesh:
+            half = np.array([e.extents.max() / 2.0 for e in self.entries])
+            s = s * (normalized_mesh_size / half[np.maximum(draw, 0)])
+        return np.where(draw >= 0, s * glob * mesh_scale, 1.0)
+
+
+def sample_object_size_scales(nenv, nslot, low, high, generator=None, device=None):
+    """exp(U(-low, high)) per environment and slot ([nenv, nslot] float64 tensor on the generator's device, else `device`): the
+    randomised object size scale of the reference (common/base.py:594-601, parameters object_scale_low / object_scale_high)."""
+    import torch
+
+    dev = generator.device if generator is not None else device
+    u = torch.rand(nenv, nslot, generator=generator, device=dev, dtype=torch.float64)
+    return torch.exp(-low + (low + high) * u)
+
 
 def _build(base_blob, library, slots, set_const):
-    """The base scene with slot k holding slots[k] = (entry index or -1, part geoms): the entry's parts, then disabled ones
-    (geom_dataid -1).  Non-object geoms keep their rows and order; meshes identical to one of the base's are shared, the
+    """The base scene with slot k holding slots[k] = (entry index or -1, part geoms, scale): the entry's parts, then disabled
+    ones (geom_dataid -1); a drawn object at scale s != 1 gets hulls scaled by s and the rows the compiler makes for them.  Non-object geoms keep their rows and order; meshes identical to one of the base's are shared, the
     others appended; the pair list is the base's, expanded from parts to slots."""
     m, names = modelblob.unpack(base_blob), modelblob.unpack_names(base_blob)
     bodies = _slot_bodies(m, names)
@@ -162,8 +217,12 @@ def _build(base_blob, library, slots, set_const):
         if k in done:
             continue
         done.add(k)
-        e, P = slots[k]
+        e, P, sc = slots[k]
         tmpl = library.entries[e] if e >= 0 else library.entries[library.identity[0][0]]
+        if e >= 0 and sc != 1.0:
+            tmpl = LibraryEntry([Hull(h.vert * sc, h.face, h.adjadr, h.adj) for h in tmpl.hulls],
+                                {f: tmpl.parts[f] * sc if f in SCALED_PART_FIELDS + ("geom_aabb",) else tmpl.parts[f] for f in PART_FIELDS},
+                                scaled_body_rows(tmpl.body, sc))
         for j in range(P):
             on = e >= 0 and j < tmpl.nparts
             for f in GEOM_ARRAYS:
@@ -235,7 +294,7 @@ def slotted_model(base_blob, library, parts_per_slot=None):
         raise ValueError(f"parts_per_slot={P} is below the library's largest object ({library.max_parts} parts)")
     m, names = modelblob.unpack(base_blob), modelblob.unpack_names(base_blob)
     ident = _base_draw(base_blob, library)
-    blob = _build(base_blob, library, [(e, P) for e in ident], set_const=False)
+    blob = _build(base_blob, library, [(e, P, 1.0) for e in ident], set_const=False)
     # every library hull, so that any draw is a change of geom_dataid rows only
     m2 = modelblob.unpack(blob)
     have = {Hull.of(m2, i).key for i in range(m2["nmesh"])}
@@ -280,13 +339,18 @@ def _base_draw(base_blob, library):
     return draw
 
 
-def compact_model(base_blob, library, draw):
-    """The model the reference builds for one draw (`draw`: a library index per slot, -1 = empty slot): each slot holds
-    exactly the drawn object's parts, and the constants mj_setConst derives are recomputed.  The identity draw gives the
-    base scene back."""
+def compact_model(base_blob, library, draw, scale=None):
+    """The model the reference builds for one draw (`draw`: a library index per slot, -1 = empty slot) with the objects at
+    `scale` (a finite scale > 0 per slot, None = all 1): each slot holds exactly the drawn object's parts, a scaled object
+    its own hulls with the vertices multiplied by its scale, and the constants mj_setConst derives are recomputed.  The
+    identity draw at scale 1 is the base scene itself, byte for byte."""
     draw = [int(e) for e in draw]
-    return _build(base_blob, library, [(e, library.entries[e].nparts if e >= 0 else 0) for e in draw],
-                  set_const=draw != _base_draw(base_blob, library))
+    scale = [1.0] * len(draw) if scale is None else [float(x) for x in np.asarray(scale, dtype=np.float64).reshape(-1)]
+    if len(scale) != len(draw) or not all(np.isfinite(x) and x > 0 for x in scale):
+        raise ValueError("compact_model: scale needs one finite value > 0 per slot")
+    if draw == _base_draw(base_blob, library) and all(s == 1.0 for s in scale):
+        return bytes(base_blob)
+    return _build(base_blob, library, [(e, library.entries[e].nparts if e >= 0 else 0, s) for e, s in zip(draw, scale)], set_const=True)
 
 
 class BatchedMeshScene:
@@ -319,7 +383,7 @@ class BatchedMeshScene:
             raise ValueError("the model lacks hulls of this library (slotted_model)") from None
         self.lowest = np.array([e.lowest_point() for e in library.entries])
         self.park_origin, self.park_pitch = park_origin, park_pitch
-        self.draw = None
+        self.draw = self.scale = None
         self._rows = {}
 
     def _row(self, name):
@@ -328,15 +392,23 @@ class BatchedMeshScene:
             self._rows[name] = np.repeat(np.asarray(self.m[name], dtype=dt).reshape(1, -1), self.sim.nenv, axis=0)
         return self._rows[name]
 
-    def set_objects(self, draw):
+    def set_objects(self, draw, scale=None):
         """draw [nenv, nslot]: a library index per environment and slot, -1 = empty slot: all parts disabled and the body keeps
         the shared model's rows, so its constants do not depend on earlier draws.  Nothing collides with an empty slot's body:
         place() parks it, and it then falls freely under gravity for the rest of the episode, so its pose and velocity are not
-        observations of anything."""
+        observations of anything.
+        scale [nenv, nslot] (finite, > 0; None = 1 everywhere): each drawn object at its own uniform scale, with the rows the
+        model compiler makes for `<mesh scale="s s s">` (module docstring) and the engine's geom_mesh_scale row = s on the slot's
+        part geoms.  Without scales the batch binds no geom_mesh_scale row (or writes ones into one bound before)."""
         draw = np.asarray(draw.cpu() if hasattr(draw, "cpu") else draw, dtype=np.int64).reshape(self.sim.nenv, self.nslot)
         if ((draw < -1) | (draw >= len(self.library.entries))).any():
             raise ValueError("draw: library indices or -1")
         nenv = self.sim.nenv
+        if scale is not None:
+            scale = np.asarray(scale.cpu() if hasattr(scale, "cpu") else scale, dtype=np.float64).reshape(nenv, self.nslot)
+            if not (np.isfinite(scale).all() and (scale > 0).all()):
+                raise ValueError("scale: finite and > 0 per environment and slot")
+            scale = np.where(draw >= 0, scale, 1.0)
         did = self._row("geom_dataid")
         grow = {f: self._row(f).reshape(nenv, self.m["ngeom"], -1) for f in SCENE_GEOM_FIELDS}
         brow = {f: self._row(f).reshape(nenv, self.m["nbody"], -1) for f in BODY_FIELDS}
@@ -354,11 +426,27 @@ class BatchedMeshScene:
                         r[:, 0] = 1.0
                     if n:
                         r[:n] = self.library.entries[e].parts[f]
-                    grow[f][envs, g0:g0 + self.P] = r
+                    if scale is not None and f in SCALED_PART_FIELDS:
+                        grow[f][envs, g0:g0 + self.P] = r[None] * scale[envs, k, None, None]
+                    else:
+                        grow[f][envs, g0:g0 + self.P] = r
                 for f in BODY_FIELDS:
-                    brow[f][envs, self.bodies[k]] = self.library.entries[e].body[f] if e >= 0 else _rows(self.m, f, "nbody")[self.bodies[k]]
-        self.draw = draw
-        for f in ("geom_dataid",) + SCENE_GEOM_FIELDS + BODY_FIELDS:
+                    if e < 0:
+                        brow[f][envs, self.bodies[k]] = _rows(self.m, f, "nbody")[self.bodies[k]]
+                    elif scale is None:
+                        brow[f][envs, self.bodies[k]] = self.library.entries[e].body[f]
+                    else:
+                        brow[f][envs, self.bodies[k]] = scaled_body_rows(self.library.entries[e].body, scale[envs, k, None])[f]
+        self.draw, self.scale = draw, scale
+        names = ("geom_dataid",) + SCENE_GEOM_FIELDS + BODY_FIELDS
+        if scale is not None or "geom_mesh_scale" in self._rows:
+            gs = self._rows.setdefault("geom_mesh_scale", np.ones((nenv, self.m["ngeom"])))
+            gs[:] = 1.0
+            if scale is not None:
+                for k in range(self.nslot):
+                    gs[:, self.geoms[k]] = scale[:, k, None]
+            names += ("geom_mesh_scale",)
+        for f in names:
             self.sim.set_param(f, self._rows[f])
         out = self.sim.set_const(fields=SET_CONST_FIELDS)
         self.sim.update_pairs()
@@ -366,8 +454,8 @@ class BatchedMeshScene:
 
     def place(self, xy, yaw, surface_z, clearance=1e-3):
         """Put the objects down: xy [nenv, nslot, 2], yaw [nenv, nslot], each drawn object resting `clearance` above
-        `surface_z` (scalar or [nenv]) by its lowest hull point; empty slots go to their parking spots on the floor, from which
-        their geom-less bodies fall freely.  Velocities zeroed."""
+        `surface_z` (scalar or [nenv]) by its lowest hull point (at the object's scale); empty slots go to their parking spots on
+        the floor, from which their geom-less bodies fall freely.  Velocities zeroed."""
         t, sim = self.t, self.sim
         dev, dt = sim.qpos.device, sim.qpos.dtype
         f = lambda v: (v if t.is_tensor(v) else t.as_tensor(np.asarray(v, dtype=np.float64))).to(device=dev, dtype=dt)
@@ -379,7 +467,10 @@ class BatchedMeshScene:
         for k in range(self.nslot):
             a, d = self.qadr[k], self.dadr[k]
             on = t.as_tensor(draw[:, k] >= 0, device=dev)
-            low = t.as_tensor(np.where(draw[:, k] >= 0, self.lowest[np.maximum(draw[:, k], 0)], 0.0), device=dev, dtype=dt)
+            low = np.where(draw[:, k] >= 0, self.lowest[np.maximum(draw[:, k], 0)], 0.0)
+            if self.scale is not None:
+                low = low * self.scale[:, k]
+            low = t.as_tensor(low, device=dev, dtype=dt)
             px = self.park_origin[0] + self.park_pitch * (k % 4)
             py = self.park_origin[1] + self.park_pitch * (k // 4)
             sim.qpos[:, a] = t.where(on, xy[:, k, 0], t.full_like(zs, px))
