@@ -181,6 +181,32 @@ int rg_set_const(rg_batch* b, const uint8_t* mask_device, void* stream);
 /* mj_resetData for the environments whose mask byte is non-zero (mask == NULL: all) */
 int rg_reset(rg_batch* b, const uint8_t* mask_device, void* stream);
 
+/* Rotated bounding boxes of object bodies, the reference's `_get_bounding_box` (get_block_bounding_box /
+ * get_mesh_bounding_box, robogym/envs/rearrange/common/utils.py:391-412): for every selected environment (mask as in
+ * rg_step_subset, NULL = all) and each of the `nsel` (<= 64) body ids in the HOST array `bodies`, the body rotated by
+ * quat[env][k] (device, fp64 [nenv][nsel][4], w x y z), out[env][k] = (center, half size) (device, fp64 [nenv][nsel][2][3]),
+ * relative to the body origin in world-aligned axes.  The box covers what the narrow phase collides with: each environment's
+ * bound geom_dataid / geom_pos / geom_quat / geom_size / mesh_scale / geom_mesh_scale rows where they are bound, the model's
+ * arrays where they are not; mesh parts with geom_dataid -1 are skipped.  Only box and mesh geoms are boxed: a selected body
+ * with any other geom is refused.  One warp per (environment, body); asynchronous on `stream`. */
+int rg_batch_body_aabb(rg_batch* b, const int* bodies, int nsel, const double* quat, const uint8_t* mask_device, double* out, void* stream);
+/* Reset-time placement of the rearrange objects, one warp per selected environment (mask as above; no model needed).
+ * Device inputs: bbox [nenv][nobj][2][3] (rg_batch_body_aabb), active [nenv][nobj] (the active objects are placed in slot
+ * order, as the reference places its num_objects; inactive slots are not written), area [nenv][6] (placement area offset,
+ * full size), anchor [nenv][nobj][3] (goal_distance_ratio only: the object placements the goals are pulled toward).  Host:
+ * table = table body pos, table geom half size.  mode 1 grid (place_objects_in_grid), 2 uniform
+ * (place_objects_with_no_constraint), 3 goal_distance_ratio (place_targets_with_goal_distance_ratio), 4 grid then uniform
+ * (RearrangeEnv._generate_object_placements); max_trials / max_per_object are the reference's max_placement_retry (also the
+ * grid's trial count) / max_placement_retry_per_object.  Out: pos [nenv][nobj][3] body-origin positions (fp64) and status
+ * [nenv]: the algorithm that succeeded (1, 2 or 3) or 0 = invalid (active slots zeroed; the reference raises
+ * InvalidSimulationError and redraws the scene, here the caller redraws those environments).  Random numbers: Philox4x32-10
+ * keyed by (seed, environment), counters (step, trial, 0, epoch) for the grid's shuffles and (proposal, 0, 1, epoch) for the
+ * samplers' proposals (robogym_b200/csrc/rg_place.inl), so results do not depend on the mask.  Asynchronous on `stream`, on
+ * the current device. */
+int rg_place_objects(int nenv, int nobj, const double* bbox, const uint8_t* active, const double table[6], const double* area, int mode,
+                     int max_trials, int max_per_object, double goal_distance_ratio, double goal_distance_min, const double* anchor,
+                     uint32_t seed, uint32_t epoch, const uint8_t* mask_device, double* pos, int* status, void* stream);
+
 const char* rg_last_error(void);
 
 #ifdef __cplusplus

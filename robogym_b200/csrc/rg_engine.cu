@@ -19,6 +19,7 @@
 
 #include "../../include/robogym_b200.h"
 #include "rg_step.inl"
+#include "rg_place.inl"
 #include "rg_host.h"
 
 #ifndef RG_MAX_WARPS
@@ -280,6 +281,42 @@ __global__ void rg_mark_kernel(const uint8_t* __restrict__ mask, uint8_t* __rest
 __global__ void rg_iota_kernel(int* order, int* cost, int* sep, int nenv) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e < nenv) { order[e] = e; cost[e] = 0; for (int i = 0; i < RG_NSEP; i++) sep[(size_t)e * RG_NSEP + i] = 0xfff; }
+}
+
+/* rg_batch_body_aabb: one warp per (environment, selected body); the lanes stride over the body's points, then a min / max
+   reduction (exact, so the result does not depend on the order) */
+struct RgAabbArgs {
+  RgModel m;
+  int nenv, nsel;
+  int body[RG_AABB_MAXSEL];
+  RgAabbRows rows;                 /* model arrays, or the first environment's bound rows ... */
+  size_t stride[6];                /* ... and the row strides (0: the model's array) of dataid, pos, quat, size, mscale, gscale */
+  const double* quat;              /* [nenv][nsel][4] */
+  const uint8_t* mask;
+  double* out;                     /* [nenv][nsel][2][3] */
+};
+__global__ void __launch_bounds__(256) rg_aabb_kernel(const __grid_constant__ RgAabbArgs a) {
+  const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (w >= a.nenv * a.nsel) return;
+  const int env = w / a.nsel, k = w - env * a.nsel;
+  if (a.mask && !a.mask[env]) return;
+  RgAabbRows r = a.rows;
+  r.dataid += env * a.stride[0]; r.pos += env * a.stride[1]; r.quat += env * a.stride[2]; r.size += env * a.stride[3];
+  if (r.mscale) r.mscale += env * a.stride[4];
+  if (r.gscale) r.gscale += env * a.stride[5];
+  double R[9], lo[3], hi[3];
+  rg_quat2mat_d(R, a.quat + (size_t)w * 4);
+  rg_aabb_lane(a.m, r, a.body[k], R, lane, lo, hi);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+    for (int c = 0; c < 3; c++) { lo[c] = fmin(lo[c], __shfl_xor_sync(0xffffffffu, lo[c], o)); hi[c] = fmax(hi[c], __shfl_xor_sync(0xffffffffu, hi[c], o)); }
+  if (lane == 0) rg_aabb_finish(lo, hi, a.out + (size_t)w * 6);
+}
+/* rg_place_objects: one warp per selected environment */
+__global__ void __launch_bounds__(128) rg_place_kernel(const __grid_constant__ RgPlaceArgs a) {
+  const int env = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (env >= a.nenv || (a.mask && !a.mask[env])) return;
+  rg_place_env(a, (uint32_t)env, threadIdx.x & 31);
 }
 
 /* ------------------------------------------------------------------ host objects */
@@ -815,6 +852,60 @@ int rg_reset(rg_batch* b, const uint8_t* mask, void* stream) {
   if (rc) return rc;
   RG_CUDA(cudaSetDevice(b->model->device));
   rg_reset_kernel<<<b->nenv, 64, 0, (cudaStream_t)stream>>>(b->model->dev, io, mask);
+  RG_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rg_batch_body_aabb(rg_batch* b, const int* bodies, int nsel, const double* quat, const uint8_t* mask, double* out, void* stream) {
+  if (!b || !bodies || !quat || !out || nsel <= 0) return rg_fail(-1, "rg_batch_body_aabb: bad argument");
+  if (nsel > RG_AABB_MAXSEL) return rg_fail(-1, "rg_batch_body_aabb: at most " + std::to_string(RG_AABB_MAXSEL) + " bodies per call");
+  const RgModel& hv = b->model->hm.view;
+  RgAabbArgs a;
+  a.m = b->model->dev;
+  a.nenv = b->nenv; a.nsel = nsel;
+  for (int k = 0; k < nsel; k++) {
+    const int body = bodies[k];
+    if (body <= 0 || body >= hv.nbody) return rg_fail(-1, "rg_batch_body_aabb: body id out of range");
+    for (int g = hv.body_geomadr[body]; g < hv.body_geomadr[body] + hv.body_geomnum[body]; g++)
+      if (hv.geom_type[g] != RG_GEOM_BOX && hv.geom_type[g] != RG_GEOM_MESH)
+        return rg_fail(-1, "rg_batch_body_aabb: body " + std::to_string(body) + " has geom " + std::to_string(g) + " of type " + std::to_string(hv.geom_type[g]) +
+                               "; only box and mesh geoms are boxed");
+    a.body[k] = body;
+  }
+  /* each environment's bound row where there is one, the model's array where there is not */
+  const char* names[6] = {"geom_dataid", "geom_pos", "geom_quat", "geom_size", "mesh_scale", "geom_mesh_scale"};
+  const void* model_ptr[6] = {a.m.geom_dataid, a.m.geom_pos, a.m.geom_quat, a.m.geom_size, nullptr, nullptr};
+  const void* ptr[6];
+  for (int i = 0; i < 6; i++) {
+    const int slot = rg_find_override(b, names[i]);
+    ptr[i] = slot >= 0 ? (const void*)b->over_ptr[slot] : model_ptr[i];
+    a.stride[i] = slot >= 0 ? (size_t)b->over_cnt[slot] : 0;
+  }
+  a.rows.dataid = (const int*)ptr[0]; a.rows.pos = (const float*)ptr[1]; a.rows.quat = (const float*)ptr[2]; a.rows.size = (const float*)ptr[3];
+  a.rows.mscale = (const float*)ptr[4]; a.rows.gscale = (const float*)ptr[5];
+  a.quat = quat; a.mask = mask; a.out = out;
+  RG_CUDA(cudaSetDevice(b->model->device));
+  const int warps = b->nenv * nsel;
+  rg_aabb_kernel<<<(warps + 7) / 8, 256, 0, (cudaStream_t)stream>>>(a);
+  RG_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rg_place_objects(int nenv, int nobj, const double* bbox, const uint8_t* active, const double table[6], const double* area, int mode,
+                     int max_trials, int max_per_object, double goal_distance_ratio, double goal_distance_min, const double* anchor,
+                     uint32_t seed, uint32_t epoch, const uint8_t* mask, double* pos, int* status, void* stream) {
+  if (nenv <= 0 || nobj <= 0 || !bbox || !active || !table || !area || !pos || !status) return rg_fail(-1, "rg_place_objects: bad argument");
+  if (nobj > RG_PLACE_MAXOBJ) return rg_fail(-1, "rg_place_objects: at most " + std::to_string(RG_PLACE_MAXOBJ) + " objects per environment");
+  if (mode < RG_PLACE_GRID || mode > RG_PLACE_GRID_THEN_UNIFORM) return rg_fail(-1, "rg_place_objects: unknown mode");
+  if (max_trials < 1 || max_per_object < 1) return rg_fail(-1, "rg_place_objects: max_trials and max_per_object must be >= 1");
+  if (mode == RG_PLACE_GOAL_DISTANCE && !anchor) return rg_fail(-1, "rg_place_objects: goal_distance_ratio needs the object placements (anchor)");
+  RgPlaceArgs a;
+  a.nenv = nenv; a.nobj = nobj; a.mode = mode; a.max_trials = max_trials; a.max_per_object = max_per_object;
+  a.ratio = goal_distance_ratio; a.dmin = goal_distance_min;
+  for (int k = 0; k < 3; k++) { a.table_pos[k] = table[k]; a.table_size[k] = table[3 + k]; }
+  a.seed = seed; a.epoch = epoch;
+  a.bbox = bbox; a.active = active; a.area = area; a.anchor = anchor; a.mask = mask; a.pos = pos; a.status = status;
+  rg_place_kernel<<<(nenv + 3) / 4, 128, 0, (cudaStream_t)stream>>>(a);
   RG_CUDA(cudaGetLastError());
   return 0;
 }

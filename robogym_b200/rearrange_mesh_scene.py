@@ -25,7 +25,7 @@ object share its library hulls, so a batch scales a part in the narrow phase wit
 """
 import numpy as np
 
-from . import mjcf, modelblob
+from . import mjcf, modelblob, rearrange_placement
 
 GEOM_MESH = 7
 # rows of a part geom that come from the library (relative to its body); geom_bodyid / geom_dataid are the slot's
@@ -479,6 +479,13 @@ class BatchedMeshScene:
             half = t.where(on, 0.5 * yaw[:, k], t.zeros_like(zs))
             sim.qpos[:, a + 3] = t.cos(half); sim.qpos[:, a + 4] = 0.0; sim.qpos[:, a + 5] = 0.0; sim.qpos[:, a + 6] = t.sin(half)
             sim.qvel[:, d:d + 6] = 0.0
+
+    def bounding_boxes(self, quat=None, mask=None):
+        """The reference's `_get_bounding_box` of every slot's object (get_mesh_bounding_box) with the object rotated by quat
+        ([nenv, nslot, 4] w x y z; None = unrotated): [nenv, nslot, 2, 3] float64 (center relative to the body origin, half size)
+        on the device, from each environment's drawn, scaled parts (rg_batch_body_aabb); an empty slot gets a zero box.  Its
+        xy feeds rearrange_placement, whose positions place() takes as they are."""
+        return rearrange_placement.body_aabb(self.sim, self.bodies, quat, mask)
 
     def set_material(self, friction=None, solref=None, solimp=None, margin=None):
         """Material rows of every part of a slot, per environment and slot: friction [nenv, nslot, 3], solref [nenv, nslot, 2],

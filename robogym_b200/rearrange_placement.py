@@ -1,0 +1,189 @@
+"""Where a rearrange reset puts the objects and their goals, for a whole batch on the device.
+
+The reference places objects from their rotated bounding boxes at every reset (`RearrangeEnv._generate_object_placements`,
+robogym/envs/rearrange/common/base.py:797-822): `place_objects_in_grid`, and when that fails the rejection sampler
+`place_objects_with_no_constraint` (100 restarts x 21 proposals per object), inside `get_placement_area`
+(simulation/base.py:992-1010).  State goals are placed the same way (`ObjectStateGoal._sample_next_goal_positions`,
+goals/object_state.py:434-457), and `TrainStateGoal` pulls each goal toward its object with
+`place_targets_with_goal_distance_ratio` (common/utils.py:922-994).
+
+Here the boxes come from `BatchedMeshScene.bounding_boxes` / `BatchedBlockScene.bounding_boxes` (`rg_batch_body_aabb`) and
+the placement from `rg_place_objects`, one warp per environment (robogym_b200/csrc/rg_place.inl), with the reference's
+semantics and defaults, draw for draw: for the same random numbers the positions are the reference's float64 results.  The
+random numbers are Philox4x32-10 keyed by (seed, environment) and addressed by an `epoch` per call, so a masked re-placement
+draws the same numbers for an environment as a full one; `PlacementSeed` hands out a fresh epoch for every call.
+
+An environment no algorithm could place comes back with status 0 (its active slots zeroed).  The reference raises
+`InvalidSimulationError` there and `safe_reset_env` rebuilds the whole scene; here the caller redraws the flagged
+environments (objects, scales, yaws) and places them again under a mask.
+
+    table = table_dimensions(model)
+    area = placement_area(table, active.sum(1), used_table_portion)
+    seed = PlacementSeed(0)
+    bbox = scene.bounding_boxes(quat)
+    pos, status = object_placements(bbox, active, table, area, *seed.next())
+"""
+import ctypes
+
+import numpy as np
+
+from . import engine, modelblob
+
+MODES = {"grid": 1, "uniform": 2, "goal_distance_ratio": 3, "grid_then_uniform": 4}
+STATUS = {0: None, 1: "grid", 2: "uniform", 3: "goal_distance_ratio"}
+# simulation/base.py:83-84, :89-90
+MAX_PLACEMENT_RETRY, MAX_PLACEMENT_RETRY_PER_OBJECT = 100, 20
+GOAL_DISTANCE_MIN = 0.06
+MAX_OBJECTS = 64
+
+_sigs = False
+
+
+def _lib():
+    global _sigs
+    L = engine.lib()
+    if not _sigs:
+        vp, ci, cd, u32 = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_uint32
+        L.rg_batch_body_aabb.argtypes = [vp, vp, ci, vp, vp, vp, vp]
+        L.rg_place_objects.argtypes = [ci, ci, vp, vp, vp, vp, ci, ci, ci, cd, cd, vp, u32, u32, vp, vp, vp, vp]
+        _sigs = True
+    return L
+
+
+def table_dimensions(model):
+    """`get_table_dimensions` (simulation/base.py:923-932): (table body pos, table geom half size, table height = size_z + pos_z),
+    float64, of a model blob (or anything with `.blob`)."""
+    blob = getattr(model, "blob", model)
+    m, names = modelblob.unpack(blob), modelblob.unpack_names(blob)
+    size = np.asarray(m["geom_size"], dtype=np.float64).reshape(-1, 3)[names["geom"].index("table")].copy()
+    pos = np.asarray(m["body_pos"], dtype=np.float64).reshape(-1, 3)[names["body"].index("table")].copy()
+    return pos, size, size[-1] + pos[-1]
+
+
+def placement_area(table, num_objects, used_table_portion=1.0):
+    """`get_placement_area` with `get_table_setting`'s clip (simulation/base.py:981-1010) per environment: num_objects is each
+    environment's active count ([nenv] or a scalar), used_table_portion a scalar or [nenv].  Returns [nenv, 6] float64
+    (offset x y z, size x y z)."""
+    _, table_size, _ = table
+    n = np.atleast_1d(np.asarray(num_objects.cpu() if hasattr(num_objects, "cpu") else num_objects))
+    used = np.asarray(used_table_portion.cpu() if hasattr(used_table_portion, "cpu") else used_table_portion, dtype=np.float64)
+    n, used = np.broadcast_arrays(n, used)
+    table_size_x, table_size_y = table_size[:2] * 2
+    used = np.clip(used, n * 0.1, 1.0)
+    place_size_x = 0.5 * table_size_x * used
+    place_size_y = 0.38 * table_size_y * used
+    out = np.empty(n.shape + (6,))
+    out[..., 0] = 0.5 * table_size_x - place_size_x / 2.0
+    out[..., 1] = 0.44 * table_size_y - place_size_y / 2.0
+    out[..., 2] = 2 * table_size[2]
+    out[..., 3], out[..., 4], out[..., 5] = place_size_x, place_size_y, 0.26
+    return out
+
+
+class PlacementSeed:
+    """A batch's placement seed and its epoch counter: every `next()` returns (seed, epoch) with a fresh epoch, so successive
+    resets draw fresh numbers."""
+
+    def __init__(self, seed=0):
+        self.seed = int(seed) & 0xFFFFFFFF
+        self.epoch = 0
+
+    def next(self):
+        e = self.epoch
+        self.epoch = (self.epoch + 1) & 0xFFFFFFFF
+        return self.seed, e
+
+
+def _dev(t, x, dtype, shape, name, device):
+    x = x if t.is_tensor(x) else t.as_tensor(np.asarray(x))
+    if tuple(x.shape) != tuple(shape):
+        try:
+            x = x.expand(*shape)
+        except RuntimeError:
+            raise ValueError(f"{name}: expected shape {tuple(shape)}, got {tuple(x.shape)}") from None
+    return x.to(device=device, dtype=dtype).contiguous()
+
+
+def _place(bbox, active, table, area, seed, epoch, mode, mask, out, max_trials, max_per_object, anchor, ratio, dmin):
+    import torch as t
+
+    if mode not in MODES:
+        raise ValueError(f"mode: one of {sorted(MODES)}")
+    if not t.is_tensor(bbox) or not bbox.is_cuda:
+        raise ValueError("bbox: a CUDA tensor [nenv, nobj, 2, 3] (bounding_boxes)")
+    if bbox.dim() != 4 or tuple(bbox.shape[2:]) != (2, 3):
+        raise ValueError("bbox: [nenv, nobj, 2, 3] (center, half size)")
+    nenv, nobj = int(bbox.shape[0]), int(bbox.shape[1])
+    if nobj > MAX_OBJECTS:
+        raise ValueError(f"at most {MAX_OBJECTS} objects per environment")
+    dev = bbox.device
+    bb = bbox.to(t.float64).contiguous()
+    if not bool(t.isfinite(bb).all()) or bool((bb[:, :, 1] < 0).any()):
+        raise ValueError("bbox: finite, with half sizes >= 0")
+    act = _dev(t, active, t.uint8, (nenv, nobj), "active", dev)
+    ar = _dev(t, area, t.float64, (nenv, 6), "area", dev)
+    tab = np.concatenate([np.asarray(table[0], dtype=np.float64).reshape(3), np.asarray(table[1], dtype=np.float64).reshape(3)])
+    if not (0 <= int(seed) < 1 << 32 and 0 <= int(epoch) < 1 << 32):
+        raise ValueError("seed and epoch: 32-bit unsigned integers")
+    if int(max_trials) < 1 or int(max_per_object) < 1:
+        raise ValueError("max_trials and max_per_object must be >= 1")
+    anc = None
+    if mode == "goal_distance_ratio":
+        if anchor is None:
+            raise ValueError("goal_distance_ratio: the object placements (anchor) are needed")
+        anc = _dev(t, anchor, t.float64, (nenv, nobj, 3), "anchor", dev)
+    mk = None if mask is None else _dev(t, mask, t.uint8, (nenv,), "mask", dev)
+    pos = t.zeros(nenv, nobj, 3, dtype=t.float64, device=dev) if out is None else out
+    if pos.dtype != t.float64 or tuple(pos.shape) != (nenv, nobj, 3) or not pos.is_contiguous() or pos.device != dev:
+        raise ValueError("out: a contiguous float64 tensor [nenv, nobj, 3] on the device of bbox")
+    status = t.full((nenv,), -1, dtype=t.int32, device=dev)
+    p = lambda x: None if x is None else ctypes.c_void_p(x.data_ptr())
+    with t.cuda.device(dev):
+        stream = ctypes.c_void_p(t.cuda.current_stream(dev).cuda_stream)
+        engine._check(_lib().rg_place_objects(nenv, nobj, p(bb), p(act), tab.ctypes.data, p(ar), MODES[mode], int(max_trials), int(max_per_object),
+                                              float(ratio), float(dmin), p(anc), int(seed), int(epoch), p(mk), p(pos), p(status), stream))
+    # (the temporaries may be freed at once: the caching allocator reuses their memory only behind the launch on this stream)
+    return pos, status
+
+
+def object_placements(bbox, active, table, area, seed, epoch, mode="grid_then_uniform", mask=None, out=None,
+                      max_trials=MAX_PLACEMENT_RETRY, max_per_object=MAX_PLACEMENT_RETRY_PER_OBJECT):
+    """Body-origin positions of the objects, `_generate_object_placements` (mode "grid_then_uniform"), or one of its parts
+    ("grid": place_objects_in_grid, "uniform": place_objects_with_no_constraint), for every environment (or those of `mask`).
+    bbox [nenv, nobj, 2, 3] (CUDA, center relative to the body origin and half size: bounding_boxes), active [nenv, nobj]
+    (placed in slot order; inactive slots are not written), table = table_dimensions(...), area [nenv, 6] (placement_area).
+    `out` ([nenv, nobj, 3] float64 CUDA) is written in place for the placed slots, so masked-out environments and inactive
+    slots keep what it held.  Returns (pos, status [nenv] int32: 1 grid, 2 uniform, 0 invalid -- redraw those environments --, -1 not selected by
+    `mask`)."""
+    return _place(bbox, active, table, area, seed, epoch, mode, mask, out, max_trials, max_per_object, None, 1.0, GOAL_DISTANCE_MIN)
+
+
+def goal_placements(bbox, active, table, area, seed, epoch, mode="goal_distance_ratio", anchor=None, goal_distance_ratio=1.0,
+                    goal_distance_min=GOAL_DISTANCE_MIN, mask=None, out=None, max_trials=MAX_PLACEMENT_RETRY,
+                    max_per_object=MAX_PLACEMENT_RETRY_PER_OBJECT):
+    """Goal positions: "goal_distance_ratio" is `TrainStateGoal` (place_targets_with_goal_distance_ratio: each goal drawn in the
+    area, then pulled toward its object's placement `anchor` [nenv, nobj, 3] to goal_distance_ratio of the distance, never
+    closer than goal_distance_min); "grid_then_uniform" is `ObjectStateGoal._sample_next_goal_positions`.  Otherwise as
+    object_placements; status 3 marks a goal-distance placement."""
+    if mode not in ("goal_distance_ratio", "grid_then_uniform"):
+        raise ValueError('goal modes: "goal_distance_ratio" or "grid_then_uniform"')
+    return _place(bbox, active, table, area, seed, epoch, mode, mask, out, max_trials, max_per_object, anchor, goal_distance_ratio, goal_distance_min)
+
+
+def body_aabb(sim, bodies, quat=None, mask=None):
+    """rg_batch_body_aabb: (center, half size) [nenv, len(bodies), 2, 3] float64 of the bodies rotated by quat
+    ([nenv, len(bodies), 4], w x y z; None = unrotated), relative to the body origin, from each environment's bound rows (the
+    model's arrays where none is bound)."""
+    t = sim.torch
+    bodies = np.ascontiguousarray(np.asarray(bodies, dtype=np.int32).reshape(-1))
+    n = len(bodies)
+    if quat is None:
+        quat = t.tensor([1.0, 0.0, 0.0, 0.0], dtype=t.float64)
+    q = _dev(t, quat, t.float64, (sim.nenv, n, 4), "quat", sim.device)
+    if not bool(t.isfinite(q).all()) or bool((q.norm(dim=2) == 0).any()):
+        raise ValueError("quat: finite and non-zero")
+    mk = None if mask is None else _dev(t, mask, t.uint8, (sim.nenv,), "mask", sim.device)
+    out = t.zeros(sim.nenv, n, 2, 3, dtype=t.float64, device=sim.device)
+    engine._check(_lib().rg_batch_body_aabb(sim.h, bodies.ctypes.data, n, ctypes.c_void_p(q.data_ptr()), None if mk is None else ctypes.c_void_p(mk.data_ptr()),
+                                            ctypes.c_void_p(out.data_ptr()), sim._stream()))
+    return out

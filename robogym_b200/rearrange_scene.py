@@ -19,7 +19,7 @@ Works on any BatchedSim-like object with `set_param` / `set_const`; the per-envi
 """
 import numpy as np
 
-from . import mjcf
+from . import mjcf, rearrange_placement
 
 GEOM_BOX = 6
 
@@ -130,6 +130,12 @@ class BatchedBlockScene:
             for g in self.geoms:
                 rows[:, g] = v
             self._push((name,))
+
+    def bounding_boxes(self, quat=None, mask=None):
+        """The reference's `_get_bounding_box` of every block (get_block_bounding_box) rotated by quat ([nenv, nobj, 4] w x y z;
+        None = unrotated): [nenv, nobj, 2, 3] float64 (center relative to the body origin, half size) on the device, from each
+        environment's size and scale rows (rg_batch_body_aabb).  Feeds rearrange_placement, whose positions place() takes."""
+        return rearrange_placement.body_aabb(self.sim, self.bodies, quat, mask)
 
     # ---- which blocks an environment uses, and where they are
     def place(self, xy, yaw, z, active=None):
