@@ -207,6 +207,57 @@ int rg_place_objects(int nenv, int nobj, const double* bbox, const uint8_t* acti
                      int max_trials, int max_per_object, double goal_distance_ratio, double goal_distance_min, const double* anchor,
                      uint32_t seed, uint32_t epoch, const uint8_t* mask_device, double* pos, int* status, void* stream);
 
+/* Rearrange goal evaluation, once per env-step: the reference's ObjectStateGoal.relative_goal / goal_distance
+ * (robogym/envs/rearrange/goals/object_state.py:492-599), RearrangeEnv._calculate_num_success /
+ * _calculate_goal_distance_reward (envs/rearrange/common/base.py:824-848), RobotEnv._is_successful (robot_env.py:569-575)
+ * and check_objects_off_table (envs/rearrange/simulation/base.py:805-832), one warp per selected environment.
+ * Inputs (device unless noted):
+ *   pos / quat: float32 object pose rows, read in place: slot k of environment e is pos[e * pos_stride + 3 * rows[k]] and
+ *     quat[e * quat_stride + 4 * rows[k]] (w x y z).  A BatchedSim's body_xpos / body_xquat with rows = body ids, or
+ *     [nenv][nobj] tensors with rows = 0..nobj-1.  rows is a HOST array of nobj (<= 64) ids.
+ *   goal_pos / goal_quat: fp64 [nenv][nobj][3|4]; group: int32 [nenv][nobj], the object's group id (duplicates share one),
+ *     -1 for an inactive (padded) slot; pos_offset / rot_weight: fp64 [nenv] (goal_pos_offset, goal_rot_weight).
+ *   table: table body pos, table geom half size (as rg_place_objects); rot_dist_type 0 full, 1 mod90, 2 mod180;
+ *   success_keys: bit 0 obj_pos, bit 1 obj_rot in success_threshold (at least one), with their thresholds.
+ * Semantics: object angles are normalize_angles(mat2euler(quat2mat(q))) (get_object_rot), goal angles mat2euler(quat2mat(q))
+ * (get_target_rot); inactive slots are zero on both sides.  Within every group of two or more active slots objects are
+ * matched to goals greedily (the first flat argmin of the position distances, repeated); the others keep their own goal.
+ * Padded slots count in num_success and goal_achieved, as in the reference.  `prev` ([nenv] fp64, in/out) holds the previous
+ * evaluation's num_success; NaN marks "none since the goal reset" and gives reward 0.  Outputs per slot: obj_rot, rel_pos,
+ * rel_rot ([nenv][nobj][3]), dist_pos, dist_rot ([nenv][nobj]), success, off_table (uint8 [nenv][nobj]); per environment:
+ * num_success (count x reward_per_object), reward (num_success - prev), achieved, any_off (uint8).  pick (optional, int32
+ * [nenv][nobj]): matched goal slot * 32 + index of the parallel quaternion taken (31: none).  fp64 with explicitly rounded
+ * operations in the reference's order (robogym_b200/csrc/rg_goal.inl).  Asynchronous on `stream`, on the current device. */
+typedef struct rg_goal_in {
+  int nenv, nobj;
+  const float* pos; const float* quat;
+  long long pos_stride, quat_stride;
+  const int* rows;
+  const double* goal_pos; const double* goal_quat;
+  const int* group;
+  const double* pos_offset; const double* rot_weight;
+  double table[6];
+  int rot_dist_type, success_keys;
+  double pos_threshold, rot_threshold, reward_per_object;
+} rg_goal_in;
+typedef struct rg_goal_out {
+  double* obj_rot; double* rel_pos; double* rel_rot;
+  double* dist_pos; double* dist_rot;
+  uint8_t* success; uint8_t* off_table;
+  double* num_success; double* reward;
+  uint8_t* achieved; uint8_t* any_off;
+  int* pick;
+} rg_goal_out;
+int rg_rearrange_goal(const rg_goal_in* in, const uint8_t* mask_device, double* prev, const rg_goal_out* out, void* stream);
+/* Goal orientations at goal reset: randomize_quaternion_along_z (mode 1: quat_mul(z_quat, base)) or randomize_quaternion_block
+ * (mode 2: quat_mul(z_quat, quat_mul(base, PARALLEL_QUATS[k]))), object_state.py:71-103, for the active slots (uint8
+ * [nenv][nobj]) of the selected environments; base = the current target quaternions (fp64 [nenv][nobj][4]), out the same
+ * shape (only those slots written; may alias base).  Random numbers: Philox4x32-10 keyed by (seed, environment); the i-th
+ * active object reads counter (i, 0, 2, epoch): words x, y give its angle uniform(0, 2 pi), word z its face index in [0, 24)
+ * (the constructions of rg_place_objects).  "full" (normal draws) is not provided. */
+int rg_goal_orientations(int nenv, int nobj, const double* base_quat, const uint8_t* active, int mode, uint32_t seed, uint32_t epoch,
+                         const uint8_t* mask_device, double* out, void* stream);
+
 const char* rg_last_error(void);
 
 #ifdef __cplusplus

@@ -20,6 +20,7 @@
 #include "../../include/robogym_b200.h"
 #include "rg_step.inl"
 #include "rg_place.inl"
+#include "rg_goal.inl"
 #include "rg_host.h"
 
 #ifndef RG_MAX_WARPS
@@ -317,6 +318,20 @@ __global__ void __launch_bounds__(128) rg_place_kernel(const __grid_constant__ R
   const int env = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (env >= a.nenv || (a.mask && !a.mask[env])) return;
   rg_place_env(a, (uint32_t)env, threadIdx.x & 31);
+}
+/* rg_rearrange_goal: one warp per selected environment, its working set in shared memory */
+#define RG_GOAL_WARPS 4
+__global__ void __launch_bounds__(32 * RG_GOAL_WARPS) rg_goal_kernel(const __grid_constant__ RgGoalArgs a) {
+  __shared__ RgGoalScratch scratch[RG_GOAL_WARPS];
+  const int w = threadIdx.x >> 5, env = blockIdx.x * RG_GOAL_WARPS + w;
+  if (env >= a.nenv || (a.mask && !a.mask[env])) return;
+  rg_goal_env(a, scratch[w], env, threadIdx.x & 31);
+}
+/* rg_goal_orientations: one warp per selected environment, a lane per slot */
+__global__ void __launch_bounds__(128) rg_goal_rot_kernel(const __grid_constant__ RgGoalRotArgs a) {
+  const int env = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (env >= a.nenv || (a.mask && !a.mask[env])) return;
+  rg_goal_rot_env(a, env, threadIdx.x & 31);
 }
 
 /* ------------------------------------------------------------------ host objects */
@@ -906,6 +921,28 @@ int rg_place_objects(int nenv, int nobj, const double* bbox, const uint8_t* acti
   a.seed = seed; a.epoch = epoch;
   a.bbox = bbox; a.active = active; a.area = area; a.anchor = anchor; a.mask = mask; a.pos = pos; a.status = status;
   rg_place_kernel<<<(nenv + 3) / 4, 128, 0, (cudaStream_t)stream>>>(a);
+  RG_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rg_rearrange_goal(const rg_goal_in* in, const uint8_t* mask, double* prev, const rg_goal_out* out, void* stream) {
+  RgGoalArgs a;
+  const char* err = rg_goal_make_args(in, mask, prev, out, a);
+  if (err) return rg_fail(-1, std::string("rg_rearrange_goal: ") + err);
+  rg_goal_kernel<<<(a.nenv + RG_GOAL_WARPS - 1) / RG_GOAL_WARPS, 32 * RG_GOAL_WARPS, 0, (cudaStream_t)stream>>>(a);
+  RG_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rg_goal_orientations(int nenv, int nobj, const double* base, const uint8_t* active, int mode, uint32_t seed, uint32_t epoch,
+                         const uint8_t* mask, double* out, void* stream) {
+  if (nenv <= 0 || nobj <= 0 || !base || !active || !out) return rg_fail(-1, "rg_goal_orientations: bad argument");
+  if (nobj > RG_GOAL_MAXOBJ) return rg_fail(-1, "rg_goal_orientations: at most " + std::to_string(RG_GOAL_MAXOBJ) + " objects per environment");
+  if (mode != RG_GOALROT_Z && mode != RG_GOALROT_BLOCK) return rg_fail(-1, "rg_goal_orientations: mode 1 z_axis or 2 block");
+  RgGoalRotArgs a;
+  a.nenv = nenv; a.nobj = nobj; a.mode = mode; a.seed = seed; a.epoch = epoch;
+  a.base = base; a.active = active; a.mask = mask; a.out = out;
+  rg_goal_rot_kernel<<<(nenv + 3) / 4, 128, 0, (cudaStream_t)stream>>>(a);
   RG_CUDA(cudaGetLastError());
   return 0;
 }
