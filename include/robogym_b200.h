@@ -258,6 +258,73 @@ int rg_rearrange_goal(const rg_goal_in* in, const uint8_t* mask_device, double* 
 int rg_goal_orientations(int nenv, int nobj, const double* base_quat, const uint8_t* active, int mode, uint32_t seed, uint32_t epoch,
                          const uint8_t* mask_device, double* out, void* stream);
 
+/* Rearrange observations, once per env-step after rg_rearrange_goal: the reference's RearrangeEnv._observe_simple with its
+ * placement-area masks (envs/rearrange/common/base.py:311-421), the robot keys of MujocoObservation
+ * (robot/ur16e/mujoco/joint_controlled_arm.py:22-85, robot/gripper/mujoco/mujoco_robotiq_gripper.py:12-35), the contact queries
+ * get_gripper_table_contact / get_wrist_cam_collisions / get_object_gripper_contact and the penalty part of
+ * _get_simulation_reward_with_done (common/base.py:768-795), one warp per selected environment.
+ * Inputs (device unless noted):
+ *   body_xpos / body_xquat / body_xvel / qpos / qvel / ctrl / sensordata / contact (float32) and ncon (int32): the main sim's
+ *     rows, read in place; each environment's row is nbody * 3 | 4 | 6, nq, nv, nu, nsensordata, ncontact * 4 floats wide.
+ *   obj_body / obj_qpos: HOST [nobj] (<= 64): body id and qpos address of the free joint of each object slot; tcp_body the
+ *     robot0:gripper_tcp body; arm_qpos the arm joints' qpos addresses (<= 8), grip_qpos / grip_qvel the gripper joints'
+ *     (<= 4), grip_act the gripper actuator; force_adr / torque_adr the sensor_adr of toolhead_force / toolhead_torque.
+ *   geom_object: int32 [ngeom], the slot whose body owns the geom (-1: none); geom_flags: uint8 [ngeom], bit 0 a geom of a
+ *     gripper body, bit 1 a robot geom (its name starts with the robot prefix); table_plane, wrist_sphere, pad[0..1]: the geoms
+ *     table_collision_plane, robot0:wrist_cam_collision_sphere, robot0:left_contact_v, robot0:right_contact_v.
+ *   goal_pos / goal_quat / rel_pos / rel_rot (fp64), achieved, off_table (uint8), group (int32, -1 inactive): the goal and the
+ *     rg_rearrange_goal outputs of the same env-step; qpos_at_goal: float32 [nenv][nq], the qpos the goal was set on.
+ *   bbox_size fp64 [nenv][nobj][3], colors fp64 [nenv][nobj][4], boundary fp64 [nenv][6] (min xyz, max xyz of the placement
+ *     area); penalty: table_collision, wrist_collision, objects_off_table, safety_stop; mask_obs, mask_margin: the
+ *     mask_obs_outside_placement_area keys (hard rule of check_objects_in_placement_area).
+ * Outputs: fp64 [nenv][...] rows under the reference's key names; inactive slots are zero (placement masks 1).  The masked_*
+ * and *_placement_mask outputs are written only with mask_obs (they may be NULL otherwise).  is_goal_achieved is int32,
+ * safety_stop, gripper_table_contact, wrist_cam_contacts ([nenv][4]: table_collision_plane, robot, object, any) and sim_done
+ * uint8.  fp64 with explicitly rounded operations in the reference's order (robogym_b200/csrc/rg_obs.inl).  Asynchronous on
+ * `stream`, on the current device. */
+typedef struct rg_obs_in {
+  int nenv, nobj;
+  const float* body_xpos; const float* body_xquat; const float* body_xvel;
+  const float* qpos; const float* qvel; const float* ctrl; const float* sensordata; const float* contact;
+  const int* ncon;
+  int nbody, nq, nv, nu, nsensordata, ncontact, ngeom;
+  const int* obj_body; const int* obj_qpos;
+  int tcp_body;
+  int narm, arm_qpos[8];
+  int ngrip, grip_qpos[4], grip_qvel[4], grip_act;
+  int force_adr, torque_adr;
+  const int* geom_object; const uint8_t* geom_flags;
+  int table_plane, wrist_sphere, pad[2];
+  const double* goal_pos; const double* goal_quat; const double* rel_pos; const double* rel_rot;
+  const uint8_t* achieved; const uint8_t* off_table; const int* group;
+  const float* qpos_at_goal;
+  const double* bbox_size; const double* colors; const double* boundary;
+  double penalty[4];
+  int mask_obs;
+  double mask_margin;
+} rg_obs_in;
+typedef struct rg_obs_out {
+  double* obj_pos; double* obj_rel_pos; double* obj_vel_pos; double* obj_rot; double* obj_vel_rot;   /* [nenv][nobj][3] */
+  double* robot_joint_pos;                                      /* [nenv][narm] */
+  double* gripper_pos; double* gripper_velp;                    /* [nenv][3] */
+  double* gripper_controls;                                     /* [nenv][1] */
+  double* gripper_qpos; double* gripper_vel;                    /* [nenv][ngrip] */
+  double* qpos; double* qpos_goal;                              /* [nenv][nq] */
+  double* goal_obj_pos; double* goal_obj_rot; double* rel_goal_obj_pos; double* rel_goal_obj_rot;   /* [nenv][nobj][3] */
+  int* is_goal_achieved;                                        /* [nenv] */
+  double* obj_gripper_contact;                                  /* [nenv][nobj][2] */
+  double* obj_bbox_size; double* obj_colors;                    /* [nenv][nobj][3 | 4] */
+  uint8_t* safety_stop;                                         /* [nenv] */
+  double* tcp_force; double* tcp_torque;                        /* [nenv][3] */
+  double* placement_mask; double* goal_placement_mask;          /* [nenv][nobj] */
+  double* masked_obj_pos; double* masked_obj_rot; double* masked_obj_rel_pos; double* masked_obj_vel_pos; double* masked_obj_vel_rot;
+  double* masked_obj_gripper_contact; double* masked_obj_bbox_size; double* masked_obj_colors;
+  double* masked_goal_obj_pos; double* masked_goal_obj_rot; double* masked_rel_goal_obj_pos; double* masked_rel_goal_obj_rot;
+  uint8_t* gripper_table_contact; uint8_t* wrist_cam_contacts;  /* [nenv], [nenv][4] */
+  double* sim_reward; uint8_t* sim_done;                        /* [nenv] */
+} rg_obs_out;
+int rg_rearrange_obs(const rg_obs_in* in, const uint8_t* mask_device, const rg_obs_out* out, void* stream);
+
 const char* rg_last_error(void);
 
 #ifdef __cplusplus

@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "librobogym_b200.so")
-DEPS = [os.path.join(SRC, f) for f in ("rg_engine.cu", "rg_defs.h", "rg_dyn.inl", "rg_col.inl", "rg_sol.inl", "rg_step.inl", "rg_place.inl", "rg_goal.inl", "rg_host.h")]
+DEPS = [os.path.join(SRC, f) for f in ("rg_engine.cu", "rg_defs.h", "rg_dyn.inl", "rg_col.inl", "rg_sol.inl", "rg_step.inl", "rg_place.inl", "rg_goal.inl", "rg_obs.inl", "rg_host.h")]
 DEPS += [os.path.join(HERE, "..", "include", f) for f in ("rg_model_fields.h", "robogym_b200.h")]
 
 

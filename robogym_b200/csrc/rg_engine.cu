@@ -21,6 +21,7 @@
 #include "rg_step.inl"
 #include "rg_place.inl"
 #include "rg_goal.inl"
+#include "rg_obs.inl"
 #include "rg_host.h"
 
 #ifndef RG_MAX_WARPS
@@ -332,6 +333,12 @@ __global__ void __launch_bounds__(128) rg_goal_rot_kernel(const __grid_constant_
   const int env = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (env >= a.nenv || (a.mask && !a.mask[env])) return;
   rg_goal_rot_env(a, env, threadIdx.x & 31);
+}
+/* rg_rearrange_obs: one warp per selected environment, no shared memory */
+__global__ void __launch_bounds__(128) rg_obs_kernel(const __grid_constant__ RgObsArgs a) {
+  const int env = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (env >= a.in.nenv || (a.mask && !a.mask[env])) return;
+  rg_obs_env(a, env, threadIdx.x & 31);
 }
 
 /* ------------------------------------------------------------------ host objects */
@@ -943,6 +950,15 @@ int rg_goal_orientations(int nenv, int nobj, const double* base, const uint8_t* 
   a.nenv = nenv; a.nobj = nobj; a.mode = mode; a.seed = seed; a.epoch = epoch;
   a.base = base; a.active = active; a.mask = mask; a.out = out;
   rg_goal_rot_kernel<<<(nenv + 3) / 4, 128, 0, (cudaStream_t)stream>>>(a);
+  RG_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rg_rearrange_obs(const rg_obs_in* in, const uint8_t* mask, const rg_obs_out* out, void* stream) {
+  RgObsArgs a;
+  const char* err = rg_obs_make_args(in, mask, out, a);
+  if (err) return rg_fail(-1, std::string("rg_rearrange_obs: ") + err);
+  rg_obs_kernel<<<(a.in.nenv + 3) / 4, 128, 0, (cudaStream_t)stream>>>(a);
   RG_CUDA(cudaGetLastError());
   return 0;
 }
