@@ -102,7 +102,10 @@ const char* rg_model_id2name(const rg_model* m, const char* objtype, int id);   
  * (1 at load; finite and > 0, else the call fails).  The narrow phase then uses the hull scaled by s about its frame origin --
  * support point s v*, with v* the support vertex of the unscaled hull -- and scales the hull's bounding box of the OBB cull
  * with it; geom_rbound (the broad phase) stays what the caller set, as in MuJoCo.  It is not part of the blob.  Editing
- * "mesh_vert" also rebuilds what the narrow phase derives from it (the padded vertex copy it scans, the geom_aabb of mesh geoms). */
+ * "mesh_vert" also rebuilds what the narrow phase derives from it (the padded vertex copy, the per-direction-cell candidate
+ * lists of the support scan, the geom_aabb of mesh geoms); a hull whose rebuilt lists outgrow the room allocated at load falls
+ * back to scanning all its vertices, with the same results.  Editing "mesh_vertadr" or "mesh_vertnum" switches every hull to
+ * that whole-hull scan. */
 int rg_model_set_field(rg_model* m, const char* name, const void* data, size_t count);
 int rg_model_set_field_async(rg_model* m, const char* name, const void* data, size_t count, void* stream);
 /* floats per environment of the RG_FIELD_DBG dump; bytes of shared memory per environment (one warp) */

@@ -131,6 +131,10 @@ __device__ __forceinline__ void rg_stage_sync() {
 #define RG_GRP 8           /* lanes that share one pair in the convex-convex narrow phase (rg_mpr_batch) */
 #endif
 #define RG_NSEP 64         /* words of the per-environment separating-axis cache (rg_mpr_batch) */
+#ifndef RG_CELLN
+#define RG_CELLN 8         /* cells per cube-face edge of the hull support lists (rg_host_hull_cells, rg_hull_cell) */
+#endif
+#define RG_NCELL (6 * RG_CELLN * RG_CELLN)   /* direction cells per hull */
 #define RG_TJ 8           /* max non-zeros of one tendon's Jacobian row */
 #ifdef RG_PROFILE
 #define RG_NPROF 16      /* per-stage cycle counters appended to the RG_DBG dump (-DRG_PROFILE builds only) */
@@ -179,6 +183,11 @@ struct RgModel {
   const float* geom_mesh_scale; /* [ngeom]: uniform scale of every mesh geom on top of its hull's mesh_scale (per-environment
                                    parameter only), or nullptr = 1 everywhere */
   const float* mesh_vert4;     /* [nmeshvert][4]: hull vertices padded to 16 bytes (one vector load each) */
+  const int* mesh_cell;        /* [nmesh][RG_NCELL][2]: (first entry in mesh_cand4, count) of every direction cell's support
+                                  candidates; count -1: scan the whole hull (rg_host_store_cells) */
+  const float* mesh_cand4;     /* [ncand][4]: candidate vertices x, y, z and the vertex id's int bits, ascending ids per cell;
+                                  right behind mesh_cell in the arena (the device finds it there: rg_hull_cands) */
+  int ncand_cap;               /* entries mesh_cand4 has room for (rebuilt lists must fit in the arena allocated at load) */
   const unsigned short* pair_packed; /* [npair] geom1 | geom2 << 8 when ngeom <= 256 (staged in shared memory), else nullptr;
                                         a view with pair_geom2 == nullptr streams an environment's own list instead (rg_pair) */
   float origin[3];             /* world translation applied at load so coordinates stay small in fp32 */
@@ -241,6 +250,7 @@ struct RgModelDev {
   RgArr<unsigned short> pair_packed;
   int has_pairs;
   const float* mesh_vert4;
+  const int* mesh_cell;        /* the candidate entries follow the table (rg_hull_cands) */
   float origin[3];
   int small_bytes;
   int nM;

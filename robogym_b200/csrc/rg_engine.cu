@@ -112,6 +112,7 @@ __global__ void __launch_bounds__(RG_MAX_WARPS * 32, 1) rg_step_kernel(const __g
     RG_SETOFF(eqrow)
     RG_SETOFF(mesh_scale)
     RG_SETPTR(mesh_vert4)
+    RG_SETPTR(mesh_cell)
     if (lane == 0) {
       sm->has_pairs = args.m.pair_packed != nullptr;
       sm->geom_mesh_scale.off = -1;   /* unbound: every factor 1 (a bound row overwrites the offset in the warp's own view) */
@@ -396,6 +397,8 @@ static void rg_wire_device_view(rg_model* mm) {
   RG_DEVPTR(eqrow)
   RG_DEVPTR(mesh_scale)
   RG_DEVPTR(mesh_vert4)
+  RG_DEVPTR(mesh_cell)
+  RG_DEVPTR(mesh_cand4)
   if (mm->hm.view.pair_packed) RG_DEVPTR(pair_packed)
 #undef RG_DEVPTR
 }
@@ -531,6 +534,19 @@ int rg_model_set_field_async(rg_model* mm, const char* name, const void* data, s
     }
     const size_t offb = (const char*)m.geom_aabb - mm->hm.arena.data();
     RG_CUDA(cudaMemcpyAsync(mm->d_arena + offb, m.geom_aabb, 24 * (size_t)m.ngeom, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  }
+  const bool vert = !strcmp(name, "mesh_vert"), layout = !strcmp(name, "mesh_vertadr") || !strcmp(name, "mesh_vertnum");
+  if (vert || layout) {
+    /* the hulls' support candidate lists follow their vertices; an edit of where the hulls are (vertadr / vertnum) switches
+       every hull to the whole-hull scan instead (count -1), which needs no list */
+    if (vert) rg_host_refresh_cells(m);
+    else {
+      m.ncand_cap = 0;
+      rg_host_store_cells(m, std::vector<int>(2 * (size_t)m.nmesh * RG_NCELL, -1), std::vector<int>());
+    }
+    const size_t offc = (const char*)m.mesh_cell - mm->hm.arena.data(), offe = (const char*)m.mesh_cand4 - mm->hm.arena.data();
+    RG_CUDA(cudaMemcpyAsync(mm->d_arena + offc, m.mesh_cell, 8 * (size_t)m.nmesh * RG_NCELL, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    if (m.ncand_cap > 0) RG_CUDA(cudaMemcpyAsync(mm->d_arena + offe, m.mesh_cand4, 16 * (size_t)m.ncand_cap, cudaMemcpyHostToDevice, (cudaStream_t)stream));
   }
   return 0;
 }

@@ -30,6 +30,117 @@ static inline void rg_host_pad_verts(RgModel& m) {
   for (int k = 0; k < m.nmeshvert; k++) { v4[4 * k] = m.mesh_vert[3 * k]; v4[4 * k + 1] = m.mesh_vert[3 * k + 1]; v4[4 * k + 2] = m.mesh_vert[3 * k + 2]; v4[4 * k + 3] = 0.0f; }
 }
 
+/* ---- support candidate lists of the hulls (the narrow phase's rg_hull_scan).
+ * The arg-max of x . d over a hull's vertices is a vertex whose normal cone holds d.  The sphere of directions is split into
+ * RG_NCELL cells, a cube map: face = axis f of the largest |d_f| and its sign s, then an RG_CELLN x RG_CELLN grid over the
+ * gnomonic coordinates (u, v) = (d_a, d_b) / |d_f| in [-1, 1]^2, a = (f + 1) % 3, b = (f + 2) % 3; cell id =
+ * ((2 f + (s < 0)) * RG_CELLN + i) * RG_CELLN + j with i from u, j from v.  Each cell lists the vertices that can win there.
+ *
+ * Invariant.  Let Q be the cell's (u, v) square dilated by RG_CELL_PAD (more than the device lookup's rounding, which is a
+ * few ulp: < 1e-6 in u), R = max |x| over the hull (vertices are centred on the hull), eps = 1e-5 R.  The list holds every
+ * vertex w with w . d >= max_x x . d - eps |d| for some d = s e_f + u e_a + v e_b, (u, v) in Q.  Any fp32 maximum of the
+ * 3-term dot the device computes is within 2 * 3 * 2^-24 R |d| < eps |d| of the exact maximum, so every vertex that ties
+ * for it is listed, and the list scan returns the lowest-id fp32 winner, as the whole-hull scan does.
+ *
+ * Construction (why it keeps the invariant).  h_w(u, v) = max_x (x - w) . d(u, v) is 2R-Lipschitz in (u, v): d moves by
+ * du e_a + dv e_b and |x - w| <= 2R.  On the dilated cell |d| <= D = sqrt(1 + umax^2 + vmax^2), so a listed vertex only needs
+ * h_w <= eps D somewhere in Q.  For a rectangle of Q with centre c and half-diagonal rho, every such w of the rectangle has
+ * h_w(c) <= eps D + 2 R rho =: tol(rho); the set S(rect) = {w : h_w(c) <= tol(rho)} therefore covers the rectangle.  The
+ * rectangle is split into quarters recursively (to RG_CELL_DEPTH levels, or until S holds one vertex) and the list is the
+ * union of the leaves' sets.  A quarter's set is a subset of its parent's (its centre is rho / 2 from the parent's, and
+ * tol(rho / 2) + 2 R rho / 2 = tol(rho)), and so is the arg-max at its centre (h = 0 there), so each set is computed over
+ * the parent's set only, with the same result as over the whole hull.  The double-precision evaluation errs by ~1e-16 R,
+ * far inside eps. */
+#define RG_CELL_PAD 1e-4
+#define RG_CELL_DEPTH 5
+struct RgCellBuild {
+  const float* v4; int nv; double R, epsD;
+  int f, a, b; double s;
+  std::vector<char> mark;
+  std::vector<std::vector<int>> pool;   /* one candidate buffer per recursion level */
+};
+static inline void rg_cell_rect(RgCellBuild& B, double u0, double u1, double v0, double v1, int depth) {
+  const std::vector<int>& par = B.pool[depth];
+  std::vector<int>& cur = B.pool[depth + 1];
+  const double uc = 0.5 * (u0 + u1), vc = 0.5 * (v0 + v1);
+  double d[3];
+  d[B.f] = B.s; d[B.a] = uc; d[B.b] = vc;
+  const double tol = B.epsD + B.R * sqrt((u1 - u0) * (u1 - u0) + (v1 - v0) * (v1 - v0));   /* eps D + 2 R rho */
+  double mx = -1e300;
+  for (int k : par) { const float* p = B.v4 + 4 * k; mx = fmax(mx, p[0] * d[0] + p[1] * d[1] + p[2] * d[2]); }
+  cur.clear();
+  for (int k : par) { const float* p = B.v4 + 4 * k; if (p[0] * d[0] + p[1] * d[1] + p[2] * d[2] >= mx - tol) cur.push_back(k); }
+  if (depth + 1 == RG_CELL_DEPTH || cur.size() <= 1) { for (int k : cur) B.mark[k] = 1; return; }
+  for (int q = 0; q < 4; q++)
+    rg_cell_rect(B, (q & 1) ? uc : u0, (q & 1) ? u1 : uc, (q & 2) ? vc : v0, (q & 2) ? v1 : vc, depth + 1);
+}
+/* candidate lists of one hull (v4: its float4-padded vertices): cells[2 c] = first entry (relative to the hull's first),
+   cells[2 c + 1] = count; the entries (ascending vertex ids per cell) are appended to `ids` */
+static inline void rg_host_hull_cells(const float* v4, int nv, int* cells, std::vector<int>& ids) {
+  RgCellBuild B;
+  B.v4 = v4; B.nv = nv; B.R = 0.0;
+  for (int k = 0; k < nv; k++) B.R = fmax(B.R, sqrt((double)v4[4 * k] * v4[4 * k] + (double)v4[4 * k + 1] * v4[4 * k + 1] + (double)v4[4 * k + 2] * v4[4 * k + 2]));
+  B.mark.assign(nv, 0);
+  B.pool.assign(RG_CELL_DEPTH + 1, std::vector<int>());
+  for (int k = 0; k < nv; k++) B.pool[0].push_back(k);
+  const size_t base = ids.size();
+  const double w = 2.0 / RG_CELLN, pad = RG_CELL_PAD;
+  for (int c = 0; c < RG_NCELL; c++) {
+    const int face = c / (RG_CELLN * RG_CELLN), i = (c / RG_CELLN) % RG_CELLN, j = c % RG_CELLN;
+    B.f = face >> 1; B.s = (face & 1) ? -1.0 : 1.0; B.a = (B.f + 1) % 3; B.b = (B.f + 2) % 3;
+    const double u0 = -1.0 + w * i - pad, u1 = -1.0 + w * (i + 1) + pad, v0 = -1.0 + w * j - pad, v1 = -1.0 + w * (j + 1) + pad;
+    const double um = fmax(fabs(u0), fabs(u1)), vm = fmax(fabs(v0), fabs(v1));
+    B.epsD = 1e-5 * B.R * sqrt(1.0 + um * um + vm * vm);
+    if (nv > 0) rg_cell_rect(B, u0, u1, v0, v1, 0);
+    cells[2 * c] = (int)(ids.size() - base);
+    for (int k = 0; k < nv; k++) if (B.mark[k]) { ids.push_back(k); B.mark[k] = 0; }
+    cells[2 * c + 1] = (int)(ids.size() - base) - cells[2 * c];
+  }
+}
+/* candidate lists of every hull (v4: float4-padded vertices of all hulls): table [nmesh][RG_NCELL][2] with model-wide entry
+   offsets, entries = vertex ids local to their hull */
+static inline void rg_host_cells(const float* v4, const int* vertadr, const int* vertnum, int nmesh, std::vector<int>& table, std::vector<int>& ids) {
+  table.assign(2 * (size_t)nmesh * RG_NCELL, 0);
+  ids.clear();
+  for (int h = 0; h < nmesh; h++) {
+    const size_t base = ids.size();
+    int* cells = table.data() + 2 * (size_t)h * RG_NCELL;
+    rg_host_hull_cells(v4 + 4 * (size_t)vertadr[h], vertnum[h], cells, ids);
+    for (int c = 0; c < RG_NCELL; c++) cells[2 * c] += (int)base;
+  }
+}
+/* write the lists into the arena (m.mesh_cell, m.mesh_cand4): a hull whose entries no longer fit in the room allocated at
+   load (an edited mesh_vert with longer lists), or that has no lists (count -1 in `table`), gets count -1 in every cell,
+   i.e. the whole-hull scan */
+static inline void rg_host_store_cells(RgModel& m, const std::vector<int>& table, const std::vector<int>& ids) {
+  int* cell = (int*)m.mesh_cell;
+  float* cand = (float*)m.mesh_cand4;
+  int used = 0;
+  for (int h = 0; h < m.nmesh; h++) {
+    const int* src = table.data() + 2 * (size_t)h * RG_NCELL;
+    int* dst = cell + 2 * (size_t)h * RG_NCELL;
+    const int first = src[0], n = src[2 * (RG_NCELL - 1)] + src[2 * (RG_NCELL - 1) + 1] - first;
+    if (n < 0 || used + n > m.ncand_cap) { for (int c = 0; c < RG_NCELL; c++) { dst[2 * c] = 0; dst[2 * c + 1] = -1; } continue; }
+    for (int c = 0; c < RG_NCELL; c++) { dst[2 * c] = src[2 * c] - first + used; dst[2 * c + 1] = src[2 * c + 1]; }
+    const int adr = m.mesh_vertadr[h];
+    for (int q = 0; q < n; q++) {
+      const int k = ids[(size_t)first + q];
+      const float* p = m.mesh_vert4 + 4 * ((size_t)adr + k);
+      float* e = cand + 4 * ((size_t)used + q);
+      e[0] = p[0]; e[1] = p[1]; e[2] = p[2];
+      memcpy(e + 3, &k, 4);
+    }
+    used += n;
+  }
+}
+
+/* after an edit of mesh_vert (mesh_vert4 re-padded first): rebuild the lists in the arena */
+static inline void rg_host_refresh_cells(RgModel& m) {
+  std::vector<int> table, ids;
+  rg_host_cells(m.mesh_vert4, m.mesh_vertadr, m.mesh_vertnum, m.nmesh, table, ids);
+  rg_host_store_cells(m, table, ids);
+}
+
 static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, std::string& err) {
   const char* p = (const char*)blob;
   if (len < 12 || memcmp(p, "RGMODEL1", 8)) { err = "bad model blob magic"; return false; }
@@ -93,6 +204,26 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
       }
     }
   }
+  /* the hulls' support candidate lists, built from the blob's vertices rounded to fp32 (the values mesh_vert4 holds) before the
+     layout, which sizes their room: what they take now plus a quarter for later mesh_vert edits (rg_host_store_cells) */
+  std::vector<int> cell_table, cell_ids;
+  {
+    size_t iv = 0, ia = 0, in = 0;
+    for (size_t i = 0; i < names.size(); i++) {
+      if (names[i] == "mesh_vert") iv = i;
+      else if (names[i] == "mesh_vertadr") ia = i;
+      else if (names[i] == "mesh_vertnum") in = i;
+    }
+    const int* va = (const int*)(p + srcoff[ia]); const int* vn = (const int*)(p + srcoff[in]);
+    for (int h = 0; h < m.nmesh; h++)
+      if (va[h] < 0 || vn[h] < 0 || va[h] > m.nmeshvert - vn[h]) { err = "mesh_vertadr / mesh_vertnum out of range"; return false; }
+    const double* sv = (const double*)(p + srcoff[iv]);
+    std::vector<float> v4(4 * (size_t)m.nmeshvert, 0.0f);
+    for (size_t k = 0; k < (size_t)m.nmeshvert; k++) for (int a = 0; a < 3; a++) v4[4 * k + a] = (float)sv[3 * k + a];
+    rg_host_cells(v4.data(), va, vn, m.nmesh, cell_table, cell_ids);
+  }
+  const size_t ncand_cap = cell_ids.size() + cell_ids.size() / 4;
+  if (ncand_cap > (size_t)0x7fffffff) { err = "hull support lists too large"; return false; }
   /* derived arrays appended to the small section would disturb the order; put them right after the blob fields
      but account for them in small_bytes by placing them BEFORE the first big field. */
   size_t first_big = names.size();
@@ -112,6 +243,8 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
   hm.small_bytes = dst;
   for (size_t i = first_big; i < names.size(); i++) { dst = rg_align16(dst); dstoff[i] = dst; dst += 4 * counts[i]; }
   dst = rg_align16(dst); const size_t off_v4 = dst; dst += 16 * (size_t)m.nmeshvert;
+  dst = rg_align16(dst); const size_t off_cell = dst; dst += 8 * (size_t)m.nmesh * RG_NCELL;
+  const size_t off_cand = dst; dst += 16 * ncand_cap;   /* right behind the table (8 * RG_NCELL is a multiple of 16): rg_hull_cands */
   dst = rg_align16(dst);
   hm.arena.assign(dst, 0);
   char* base = hm.arena.data();
@@ -258,6 +391,13 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
     m.pair_packed = pk;
   }
   hm.offsets.push_back(off_v4);
+  /* the hulls' support candidate lists (global memory, behind the staged section: shared memory per CTA is unchanged) */
+  m.mesh_cell = (const int*)(base + off_cell);
+  m.mesh_cand4 = (const float*)(base + off_cand);
+  m.ncand_cap = (int)ncand_cap;
+  rg_host_store_cells(m, cell_table, cell_ids);
+  hm.offsets.push_back(off_cell);
+  hm.offsets.push_back(off_cand);
   /* fp32 conditioning: translate the world so the scene sits near the origin */
   double o[3] = {0, 0, 0};
   int cnt = 0;

@@ -72,7 +72,7 @@ def main():
            "exit:gradient", "exit:alpha", "exit:improvement"]
     for k, l in enumerate(lab):
         print("%-22s %10d  per forward %.3f" % (l, x[k], x[k] / fw))
-    print("support calls per forward %.2f, climb steps %.2f, mpr pairs %.2f (hits %.2f)" % (s[0] / fw, s[1] / fw, s[2] / fw, s[3] / fw))
+    print("support calls per forward %.2f, hull vertices visited %.2f, mpr pairs %.2f (hits %.2f)" % (s[0] / fw, s[1] / fw, s[2] / fw, s[3] / fw))
     h = s[8:136].reshape(2, 64)
     print("mpr iteration histogram (miss):", h[0][:24])
     print("mpr iteration histogram (hit): ", h[1][:40])
