@@ -1,36 +1,82 @@
-"""ctypes front end of the CPU emulation build of the CUDA device code (tests only)."""
+"""ctypes front end of the CPU emulation build of the CUDA device code (tests only): tests/emu/_build/librg_emu.so, made on first
+use.  RG_EMU_LIB names another build of tests/emu/rg_emu.cpp (e.g. tools/emu_stats.py's -DRG_STATS one), loaded as it is."""
 import ctypes
 import os
 import subprocess
 
 import numpy as np
 
+from robogym_b200 import rearrange_goal as rg
+from robogym_b200 import rearrange_obs as ro
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = os.path.join(_HERE, "_build", "librg_emu.so")
+_ENV_LIB = os.environ.get("RG_EMU_LIB")
 NCON = 32
 CON_STRIDE = 24
 _lib = None
 
 
 def lib():
+    """the emulation library, with argtypes and restype of every entry point"""
     global _lib
     if _lib is None:
-        subprocess.check_call(["make", "-C", _HERE, "-s"])
-        L = ctypes.CDLL(_LIB)
-        L.rge_create_ex.restype = ctypes.c_void_p
-        L.rge_create_ex.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_int, ctypes.c_int, ctypes.c_int]
-        L.rge_destroy.argtypes = [ctypes.c_void_p]
+        if _ENV_LIB is None:
+            subprocess.check_call(["make", "-C", _HERE, "-s", "_build/librg_emu.so"])
+        L = ctypes.CDLL(_ENV_LIB or os.path.join(_HERE, "_build", "librg_emu.so"))
+        vp, ci, cd, u32 = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_uint32
+        pi = ctypes.POINTER(ctypes.c_int)
+        # handles and the step
+        L.rge_create_ex.restype = vp
+        L.rge_create_ex.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ci, ci, ci]
+        L.rge_destroy.argtypes = [vp]
         for f in ("rge_dbg_size", "rge_scratch_floats", "rge_small_bytes", "rge_ncon", "rge_pidw"):
-            getattr(L, f).argtypes = [ctypes.c_void_p]
-        L.rge_name2id.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_char_p]
-        L.rge_model_field.restype = ctypes.c_void_p
-        L.rge_model_field.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_int)]
-        L.rge_set_const.argtypes = [ctypes.c_void_p] + [ctypes.c_void_p] * 6
-        L.rge_set_sensordata.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-        L.rge_set_mocap.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-        L.rge_step.argtypes = [ctypes.c_void_p, ctypes.c_int] + [ctypes.c_void_p] * 18 + [ctypes.c_int, ctypes.c_int]
+            getattr(L, f).argtypes = [vp]
+        L.rge_name2id.argtypes = [vp, ctypes.c_char_p, ctypes.c_char_p]
+        L.rge_model_field.restype = vp
+        L.rge_model_field.argtypes = [vp, ctypes.c_char_p, pi]
+        L.rge_set_const.argtypes = [vp] + [vp] * 6
+        L.rge_set_sensordata.argtypes = [vp, vp]
+        L.rge_set_mocap.argtypes = [vp, vp, vp]
+        L.rge_step.argtypes = [vp, ci] + [vp] * 18 + [ci, ci]
+        # a handle's model view: mesh scale, pair lists, geom scale
+        L.rge_mesh_scale.restype = vp
+        L.rge_mesh_scale.argtypes = [vp, pi]
+        L.rge_pairs.argtypes = [vp, vp, vp, ci, pi]
+        L.rge_use_pairs.argtypes = [vp, vp, ci]
+        L.rge_use_geom_scale.argtypes = [vp, vp]
+        # hull support mapping
+        L.rge_support_table.restype = vp
+        L.rge_support_table.argtypes = [vp]
+        L.rge_support_entries.restype = vp
+        L.rge_support_entries.argtypes = [vp, pi]
+        L.rge_support_cell.argtypes = [vp]
+        L.rge_support_scan.argtypes = [vp, ci, vp, ci, vp]
+        L.rge_support_set_vert.argtypes = [vp, vp]
+        L.rge_support_build_seconds.restype = cd
+        L.rge_support_build_seconds.argtypes = [vp]
+        # placement
+        L.rge_philox.argtypes = [ci, vp, u32, u32, vp]
+        L.rge_body_aabb.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp]
+        L.rge_place.argtypes = [ci, ci, vp, vp, vp, vp, ci, ci, ci, cd, cd, vp, u32, u32, vp, vp, vp]
+        # goal evaluation and goal orientations
+        L.rge_goal.argtypes = [ctypes.POINTER(rg.GoalIn), vp, vp, ctypes.POINTER(rg.GoalOut)]
+        L.rge_goal_error.restype = ctypes.c_char_p
+        L.rge_goal_rot.argtypes = [ci, ci, vp, vp, ci, u32, u32, vp, vp]
+        L.rge_parallel_quats.argtypes = [vp]
+        # rearrange observations
+        L.rge_obs.argtypes = [ctypes.POINTER(ro.ObsIn), vp, ctypes.POINTER(ro.ObsOut)]
+        L.rge_obs_error.restype = ctypes.c_char_p
         _lib = L
     return _lib
+
+
+def philox_check():
+    """the sm_90a check of the device Philox against cuRAND's (needs a GPU): rg_philox_mismatches(n, k0, k1)"""
+    subprocess.check_call(["make", "-C", _HERE, "-s", "_build/librg_philox_check.so"])
+    L = ctypes.CDLL(os.path.join(_HERE, "_build", "librg_philox_check.so"))
+    L.rg_philox_mismatches.restype = ctypes.c_longlong
+    L.rg_philox_mismatches.argtypes = [ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32]
+    return L
 
 
 def _p(a):
@@ -75,6 +121,24 @@ class EmuBatch:
         p = lib().rge_model_field(self.h, name.encode(), ctypes.byref(n))
         ct = ctypes.c_int32 if dtype == np.int32 else ctypes.c_float
         return np.frombuffer((ct * n.value).from_address(p), dtype=dtype)
+
+    def mesh_scale(self):
+        """writable float32 view of the model's [nmesh] mesh_scale (engine-derived, so model_field does not serve it)"""
+        n = ctypes.c_int()
+        p = lib().rge_mesh_scale(self.h, ctypes.byref(n))
+        return np.frombuffer((ctypes.c_float * n.value).from_address(p), dtype=np.float32)
+
+    def use_pairs(self, pairs, n):
+        """step the first n pairs of `pairs` (packed g1 | g2 << 16) instead of the model's static list, as the engine does for an
+        environment with its own list; the batch keeps the array alive"""
+        self._pairs = np.ascontiguousarray(pairs, dtype=np.uint32)
+        lib().rge_use_pairs(self.h, _p(self._pairs), n)
+
+    def use_geom_scale(self, row):
+        """step with the [ngeom] geom_mesh_scale row (None: unbound, every factor 1), as the engine binds it per environment; the
+        batch keeps the array alive.  Returns ngeom."""
+        self._geom_scale = None if row is None else np.ascontiguousarray(row, dtype=np.float32)
+        return lib().rge_use_geom_scale(self.h, _p(self._geom_scale))
 
     def step(self, nsub, final_forward=1):
         lib().rge_set_mocap(self.h, _p(self.mocap_pos), _p(self.mocap_quat))

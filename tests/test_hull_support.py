@@ -8,7 +8,6 @@ import ctypes
 import glob
 import hashlib
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -18,26 +17,6 @@ from robogym_b200 import modelblob
 
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 ASSETS = sorted(glob.glob(os.path.join(ROOT, "robogym_b200", "assets", "*.rgm")))
-_lib = None
-
-
-def lib():
-    global _lib
-    if _lib is None:
-        here = os.path.join(ROOT, "tests", "emu_support")
-        subprocess.check_call(["make", "-C", here, "-s"])
-        L = ctypes.CDLL(os.path.join(here, "_build", "librg_emu_support.so"))
-        L.rge_support_table.restype = ctypes.c_void_p
-        L.rge_support_table.argtypes = [ctypes.c_void_p]
-        L.rge_support_entries.restype = ctypes.c_void_p
-        L.rge_support_entries.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int)]
-        L.rge_support_cell.argtypes = [ctypes.c_void_p]
-        L.rge_support_scan.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
-        L.rge_support_set_vert.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-        L.rge_support_build_seconds.restype = ctypes.c_double
-        L.rge_support_build_seconds.argtypes = [ctypes.c_void_p]
-        _lib = L
-    return _lib
 
 
 def _batch(blob, m):
@@ -46,7 +25,7 @@ def _batch(blob, m):
 
 def lists(e, nmesh):
     """(table [nmesh][ncell][2], entries [used][4] float32 with the vertex ids in column 3 as int32 bits)"""
-    L = lib()
+    L = pyemu.lib()
     nc = L.rge_support_ncell()
     tab = np.frombuffer((ctypes.c_int32 * (2 * nmesh * nc)).from_address(L.rge_support_table(e.h)), dtype=np.int32).reshape(nmesh, nc, 2).copy()
     cap = ctypes.c_int()
@@ -59,7 +38,7 @@ def lists(e, nmesh):
 def scan(e, mesh, dirs):
     d = np.ascontiguousarray(dirs, dtype=np.float32).reshape(-1, 3)
     out = np.zeros((len(d), 4), np.int32)
-    lib().rge_support_scan(e.h, mesh, d.ctypes.data, len(d), out.ctypes.data)
+    pyemu.lib().rge_support_scan(e.h, mesh, d.ctypes.data, len(d), out.ctypes.data)
     return out
 
 
@@ -102,7 +81,7 @@ def _edge_dirs(N, rng, per_line=64):
 def test_cell_lookup():
     """rg_hull_cell: face = largest |component| and its sign, then the N x N grid of (d_a, d_b) / |d_f|; -1 (whole-hull scan)
     for zero, tiny, huge and non-finite directions"""
-    L = lib()
+    L = pyemu.lib()
     N = L.rge_support_celln()
     rng = np.random.RandomState(3)
     d = rng.randn(20000, 3).astype(np.float32)
@@ -132,7 +111,7 @@ def test_cell_scan_matches_whole_hull_scan(asset, mesh):
     F = m["mesh_face"].reshape(-1, 3)[fa:fa + fn]
     normals = np.cross(V[F[:, 1]] - V[F[:, 0]], V[F[:, 2]] - V[F[:, 0]]).astype(np.float32)
     axes = np.array([(i, j, k) for i in (-1, 0, 1) for j in (-1, 0, 1) for k in (-1, 0, 1) if (i, j, k) != (0, 0, 0)], np.float32)
-    N = lib().rge_support_celln()
+    N = pyemu.lib().rge_support_celln()
     sets = {"random": rng.randn(100000, 3).astype(np.float32), "face normals": np.concatenate([normals, -normals]),
             "axes and diagonals": np.concatenate([axes, 0.01 * axes, 7.0 * axes]), "cell edges and corners": _edge_dirs(N, rng)}
     for name, d in sets.items():
@@ -152,7 +131,7 @@ def test_cell_scan_matches_whole_hull_scan(asset, mesh):
 
 def test_list_sizes_and_build_time():
     """the lists stay short (the scan's point) and their construction cheap at model load"""
-    L = lib()
+    L = pyemu.lib()
     for path in ASSETS:
         blob = open(path, "rb").read()
         m = modelblob.unpack(blob)
@@ -192,7 +171,7 @@ def test_mesh_vert_edit_rebuilds_lists(asset):
     blob2 = modelblob.pack(edited, modelblob.unpack_names(blob))
     e1, e2 = _batch(blob, m), _batch(blob2, m)
     v = np.ascontiguousarray(verts, dtype=np.float64)
-    lib().rge_support_set_vert(e1.h, v.ctypes.data)
+    pyemu.lib().rge_support_set_vert(e1.h, v.ctypes.data)
     e1.model_field("geom_aabb", np.float32)[:] = np.asarray(edited["geom_aabb"], dtype=np.float32)
     t1, n1 = lists(e1, m["nmesh"])
     t2, n2 = lists(e2, m["nmesh"])

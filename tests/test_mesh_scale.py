@@ -4,11 +4,9 @@ built on it (FullCubeRandomizer(cube_size_range=...), the reference's Randomized
 The oracle carries the reference's literal edits: mesh_vert x s, geom_rbound x s, cubelet body_pos x s.  The engine keeps the
 vertices and scales the support point (and its own OBB cull box) by mesh_scale instead."""
 import copy
-import ctypes
 import gzip
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -20,23 +18,6 @@ from robogym_b200 import mjcf, modelblob
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 CAPS = dict(contact_capacity=64, row_capacity=256, dofs_per_contact=32)
 CONSTS = ("dof_invweight0", "body_invweight0", "tendon_invweight0", "tendon_length0", "body_subtreemass", "opt_meaninertia")
-_scale_lib = None
-
-
-def emu_mesh_scale(e):
-    """writable float32 view of the emulated model's mesh_scale array (an engine-derived array, not a blob field: reached through
-    tests/emu_scale, which reads the emulation handle)"""
-    global _scale_lib
-    if _scale_lib is None:
-        here = os.path.join(ROOT, "tests", "emu_scale")
-        subprocess.check_call(["make", "-C", here, "-s"])
-        L = ctypes.CDLL(os.path.join(here, "_build", "librg_emu_scale.so"))
-        L.rge_mesh_scale.restype = ctypes.c_void_p
-        L.rge_mesh_scale.argtypes = [ctypes.c_void_p, ctypes.POINTER(ctypes.c_int)]
-        _scale_lib = L
-    n = ctypes.c_int()
-    p = _scale_lib.rge_mesh_scale(e.h, ctypes.byref(n))
-    return np.frombuffer((ctypes.c_float * n.value).from_address(p), dtype=np.float32)
 
 
 # ---------------------------------------------------------------------------------------------- small model with hulls
@@ -77,7 +58,7 @@ def _scale_oracle(om, m, s):
 
 
 def _scale_emu(e, m, s):
-    emu_mesh_scale(e)[:] = s
+    e.mesh_scale()[:] = s
     e.model_field("geom_rbound", np.float32)[_mesh_geoms(m)] *= np.float32(s)
 
 
@@ -130,7 +111,7 @@ def test_explicit_unit_mesh_scale_is_bit_identical():
     for explicit in (False, True):
         e = pyemu.EmuBatch(blob, dims, 1)
         if explicit:
-            emu_mesh_scale(e)[:] = 1.0
+            e.mesh_scale()[:] = 1.0
         e.qpos[0], e.qvel[0], e.warm[0] = d.qpos, d.qvel, d.qacc_warmstart
         for _ in range(10):
             e.step(5, 1)
@@ -286,7 +267,7 @@ def test_emulated_full_cube_at_scale_1_05(full_states):
     e = pyemu.EmuBatch(blob, {k: m[k] for k in modelblob.DIMS}, n, **CAPS)
     e.model_field("body_pos", np.float32)[:] = _host_shifted_body_pos(blob, edited["body_pos"])
     e.model_field("geom_rbound", np.float32)[:] = edited["geom_rbound"]
-    emu_mesh_scale(e)[mid] = 1.05
+    e.mesh_scale()[mid] = 1.05
     for k in CONSTS:
         if np.asarray(edited[k]).size:
             e.model_field(k, np.float32)[:] = np.asarray(edited[k]).reshape(-1)

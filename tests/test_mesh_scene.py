@@ -4,7 +4,6 @@ per-environment geom_dataid rows and pair lists (rg_batch_update_pairs) that mak
 step."""
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -19,7 +18,6 @@ ASSETS = os.path.join(ROOT, "robogym_b200", "assets")
 ARM_INIT = np.deg2rad(np.array([135.0, -90.0, 135.0, -100.0, -240.0, 135.0]))   # robogym/robot/ur16e/arm_interface.py:27
 TABLE_TOP = 0.453 + 0.03324
 CAPS = dict(contact_capacity=64, row_capacity=128)
-_mesh_lib = None
 
 
 def _blob(name):
@@ -31,19 +29,6 @@ def scene():
     b8, bt = _blob("rearrange_ycb8"), _blob("rearrange_ycb8_tcp")
     lib = rms.ObjectLibrary.from_blobs(b8, bt)
     return b8, lib, rms.slotted_model(b8, lib)
-
-
-def emu_pairs_lib():
-    """tests/emu_mesh: the device code's pair-list compaction, and per-environment lists on an emulation handle"""
-    global _mesh_lib
-    if _mesh_lib is None:
-        here = os.path.join(ROOT, "tests", "emu_mesh")
-        subprocess.check_call(["make", "-C", here, "-s"])
-        L = ctypes.CDLL(os.path.join(here, "_build", "librg_emu_mesh.so"))
-        L.rge_pairs.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(ctypes.c_int)]
-        L.rge_use_pairs.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
-        _mesh_lib = L
-    return _mesh_lib
 
 
 def _active_pairs(m, dataid):
@@ -113,7 +98,7 @@ def test_emulated_pair_compaction_matches_the_host_rule(scene):
     b8, lib, sb = scene
     ms = modelblob.unpack(sb)
     e = pyemu.EmuBatch(sb, {k: ms[k] for k in modelblob.DIMS}, 1)
-    L = emu_pairs_lib()
+    L = pyemu.lib()
     rng = np.random.RandomState(3)
     for draw in ([2] * 8, list(rng.randint(0, len(lib.entries), 8))):
         rows, _ = _scene_rows(sb, lib, np.array([draw]))
@@ -307,14 +292,12 @@ def _emu_scene(sb, lib, draw, nenv):
     for k, v in e.set_const().items():
         if k in rms.SET_CONST_FIELDS:
             e.model_field(k, np.float32)[:] = v
-    L = emu_pairs_lib()
     lst = np.zeros(ms["npair"], np.uint32)
     w = ctypes.c_int()
     did = rows["geom_dataid"][0].astype(np.int32)
-    n = L.rge_pairs(e.h, did.ctypes.data, lst.ctypes.data, len(lst), ctypes.byref(w))
+    n = pyemu.lib().rge_pairs(e.h, did.ctypes.data, lst.ctypes.data, len(lst), ctypes.byref(w))
     assert w.value == 0
-    L.rge_use_pairs(e.h, lst.ctypes.data, n)
-    e._pairs = lst                                         # alive as long as the batch
+    e.use_pairs(lst, n)
     return e
 
 

@@ -4,11 +4,9 @@ on top of it `BatchedMeshScene.set_objects(draw, scale)`, `compact_model(..., sc
 
 The ground truth of what the reference compiles for a scaled object is tests/golden/reference_ycb_scale.json.gz, written by
 tools/make_ycb_scale_golden.py from the reference's own make_mesh_object documents and STL files."""
-import ctypes
 import gzip
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -22,7 +20,6 @@ from robogym_b200 import rearrange_mesh_scene as rms
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_ycb_scale.json.gz")
 TABLE_TOP, CAPS, ARM_INIT = tms.TABLE_TOP, tms.CAPS, tms.ARM_INIT
-_geom_scale_lib = None
 
 
 @pytest.fixture(scope="module")
@@ -35,18 +32,6 @@ def scene():
 @pytest.fixture(scope="module")
 def golden():
     return json.loads(gzip.decompress(open(GOLDEN, "rb").read()))
-
-
-def emu_geom_scale_lib():
-    """tests/emu_geom_scale: point an emulation handle's geom_mesh_scale at a caller-owned [ngeom] row (or NULL)"""
-    global _geom_scale_lib
-    if _geom_scale_lib is None:
-        here = os.path.join(ROOT, "tests", "emu_geom_scale")
-        subprocess.check_call(["make", "-C", here, "-s"])
-        L = ctypes.CDLL(os.path.join(here, "_build", "librg_emu_geom_scale.so"))
-        L.rge_use_geom_scale.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
-        _geom_scale_lib = L
-    return _geom_scale_lib
 
 
 def _scene_rows(sb, lib, draw, scale):
@@ -318,8 +303,8 @@ def _emu_scene(sb, lib, draw, scale, nenv, bind=True):
     for k, v in e.set_const().items():
         if k in rms.SET_CONST_FIELDS:
             e.model_field(k, np.float32)[:] = v
-    e._geom_scale = rows["geom_mesh_scale"][0].astype(np.float32)      # alive as long as the batch
-    assert emu_geom_scale_lib().rge_use_geom_scale(e.h, e._geom_scale.ctypes.data if bind else None) == len(e._geom_scale)
+    row = rows["geom_mesh_scale"][0]
+    assert e.use_geom_scale(row if bind else None) == len(row)
     return e
 
 

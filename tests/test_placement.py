@@ -3,12 +3,10 @@ object bodies (rg_batch_body_aabb) and the reference's grid, rejection and goal-
 
 The fixture tests/golden/reference_placement.json.gz holds the reference's own results (tools/make_placement_golden.py), drawn
 from the same Philox counters as the kernel through a replay RandomState (tests/placement_rng.py).  The CPU tier runs the
-kernel's code on the emulation build (tests/emu_place); the GPU tier runs it on the device."""
-import ctypes
+kernel's code on the emulation build (tests/emu); the GPU tier runs it on the device."""
 import gzip
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -24,28 +22,13 @@ ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_placement.json.gz")
 ASSETS = os.path.join(ROOT, "robogym_b200", "assets")
 MODES = rp.MODES
-_emu = None
-
-
-def emu():
-    global _emu
-    if _emu is None:
-        here = os.path.join(ROOT, "tests", "emu_place")
-        subprocess.check_call(["make", "-C", here, "-s", "_build/librg_emu_place.so"])
-        L = ctypes.CDLL(os.path.join(here, "_build", "librg_emu_place.so"))
-        vp, ci, cd, u32 = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_uint32
-        L.rge_philox.argtypes = [ci, vp, u32, u32, vp]
-        L.rge_body_aabb.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp]
-        L.rge_place.argtypes = [ci, ci, vp, vp, vp, vp, ci, ci, ci, cd, cd, vp, u32, u32, vp, vp, vp]
-        _emu = L
-    return _emu
 
 
 def _ptr(a):
     return None if a is None else a.ctypes.data
 
 
-def emu_place(bbox, active, table, area, mode, seed, epoch, anchor=None, ratio=1.0, dmin=0.06, mask=None, pos=None, max_trials=100, max_per_object=20):
+def emulated_place(bbox, active, table, area, mode, seed, epoch, anchor=None, ratio=1.0, dmin=0.06, mask=None, pos=None, max_trials=100, max_per_object=20):
     """the kernel's code on the emulation build: (pos [nenv, nobj, 3], status [nenv]; -1 where mask is 0)"""
     bbox = np.ascontiguousarray(bbox, dtype=np.float64)
     nenv, nobj = bbox.shape[:2]
@@ -56,8 +39,8 @@ def emu_place(bbox, active, table, area, mode, seed, epoch, anchor=None, ratio=1
     mask = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
     pos = np.zeros((nenv, nobj, 3)) if pos is None else pos
     status = np.full(nenv, -1, np.int32)
-    emu().rge_place(nenv, nobj, _ptr(bbox), _ptr(active), _ptr(table), _ptr(area), MODES[mode], max_trials, max_per_object, ratio, dmin,
-                    _ptr(anchor), seed, epoch, _ptr(mask), _ptr(pos), _ptr(status))
+    pyemu.lib().rge_place(nenv, nobj, _ptr(bbox), _ptr(active), _ptr(table), _ptr(area), MODES[mode], max_trials, max_per_object, ratio, dmin,
+                          _ptr(anchor), seed, epoch, _ptr(mask), _ptr(pos), _ptr(status))
     return pos, status
 
 
@@ -105,7 +88,7 @@ def test_philox_known_answers_and_replay_equals_emulated_device_philox():
     ctr = rng.randint(0, 1 << 32, (4096, 4), dtype=np.uint64).astype(np.uint32)
     for k0, k1 in ((0, 0), (12345, 77), (0xFFFFFFFF, 4095)):
         out = np.zeros_like(ctr)
-        emu().rge_philox(len(ctr), _ptr(ctr), k0, k1, _ptr(out))
+        pyemu.lib().rge_philox(len(ctr), _ptr(ctr), k0, k1, _ptr(out))
         assert np.array_equal(out, philox(ctr, k0, k1))
 
 
@@ -124,7 +107,7 @@ def test_emulated_kernel_reproduces_every_reference_case(golden):
     modes = set()
     for i, c in enumerate(golden["cases"]):
         bbox, active, area, anchor, mask = _case_inputs(c)
-        pos, st = emu_place(bbox, active, golden["table"], area, c["mode"], c["seed"], c["epoch"], anchor, c["ratio"], c["dmin"], mask)
+        pos, st = emulated_place(bbox, active, golden["table"], area, c["mode"], c["seed"], c["epoch"], anchor, c["ratio"], c["dmin"], mask)
         assert st[-1] == c["status"], (i, c["mode"], st[-1], c["status"])
         assert np.abs(pos[-1] - np.array(c["pos"])).max() <= 1e-12, (i, pos[-1] - np.array(c["pos"]))
         assert (st[:-1] == -1).all() and not pos[:-1].any()
@@ -151,7 +134,7 @@ def test_placement_area_matches_the_reference(golden):
 
 def test_emulated_boxes_match_the_reference_boxes(golden, ycb):
     b8, lib, sb = ycb
-    L = emu()
+    L = pyemu.lib()
     yawq = lambda a: np.array([np.cos(0.5 * a), 0.0, 0.0, np.sin(0.5 * a)])
     nmesh = 0
     for b in golden["boxes"]:
@@ -201,9 +184,9 @@ def test_emulated_placements_hold_the_reference_invariants(mode):
     area = rp.placement_area((table[:3], table[3:], top), active.sum(1), rng.uniform(0.4, 1.0, nenv))
     anchor = None
     if mode == "goal_distance_ratio":
-        anchor, st0 = emu_place(bbox, active, table, area, "uniform", 5, 0)
+        anchor, st0 = emulated_place(bbox, active, table, area, "uniform", 5, 0)
     init = np.full((nenv, nobj, 3), 7.0)
-    pos, st = emu_place(bbox, active, table, area, mode, int(rng.randint(1 << 31)), 3, anchor, 0.5, 0.06, pos=init.copy())
+    pos, st = emulated_place(bbox, active, table, area, mode, int(rng.randint(1 << 31)), 3, anchor, 0.5, 0.06, pos=init.copy())
     assert (st >= 0).all() and (st > 0).mean() > 0.5
     assert np.array_equal(pos[~active], init[~active])
     for e in np.nonzero(st > 0)[0]:
@@ -227,10 +210,10 @@ def test_emulated_masked_call_changes_only_the_masked_environments():
     table = np.array([1.3, 0.75, 0.2, 0.6075, 0.7655, 0.2])
     bbox = _random_boxes(rng, nenv, nobj, 0.02, 0.05)
     area = rp.placement_area((table[:3], table[3:], 0.4), nobj, 1.0)
-    full, st = emu_place(bbox, 1, table, area, "grid_then_uniform", 11, 4)
+    full, st = emulated_place(bbox, 1, table, area, "grid_then_uniform", 11, 4)
     mask = rng.rand(nenv) < 0.3
     before = rng.uniform(size=(nenv, nobj, 3))
-    part, st2 = emu_place(bbox, 1, table, area, "grid_then_uniform", 11, 4, mask=mask, pos=before.copy())
+    part, st2 = emulated_place(bbox, 1, table, area, "grid_then_uniform", 11, 4, mask=mask, pos=before.copy())
     assert np.array_equal(part[mask], full[mask]) and np.array_equal(part[~mask], before[~mask])
     assert np.array_equal(st2[mask], st[mask]) and (st2[~mask] == -1).all()
 
@@ -261,11 +244,7 @@ def _gpu_place(bbox, active, table, area, mode, seed, epoch, anchor=None, ratio=
 
 @pytest.mark.gpu
 def test_cuda_philox_equals_curand_on_a_million_counters():
-    here = os.path.join(ROOT, "tests", "emu_place")
-    subprocess.check_call(["make", "-C", here, "-s", "_build/librg_philox_check.so"])
-    L = ctypes.CDLL(os.path.join(here, "_build", "librg_philox_check.so"))
-    L.rg_philox_mismatches.restype = ctypes.c_longlong
-    L.rg_philox_mismatches.argtypes = [ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32]
+    L = pyemu.philox_check()
     for k0, k1 in ((0, 0), (20261016, 1023), (0xFFFFFFFF, 0xDEADBEEF)):
         assert L.rg_philox_mismatches(1 << 20, k0, k1) == 0
 
@@ -288,8 +267,8 @@ def test_cuda_kernel_equals_emulation_and_masked_calls_touch_only_the_masked(mod
     bbox = _random_boxes(rng, nenv, nobj, 0.01, 0.08)
     active = rng.rand(nenv, nobj) < 0.8
     area = rp.placement_area((table[:3], table[3:], 0.4), active.sum(1), rng.uniform(0.4, 1.0, nenv))
-    anchor = emu_place(bbox, active, table, area, "uniform", 2, 0)[0] if mode == "goal_distance_ratio" else None
-    want, wst = emu_place(bbox, active, table, area, mode, 99, 7, anchor, 0.5)
+    anchor = emulated_place(bbox, active, table, area, "uniform", 2, 0)[0] if mode == "goal_distance_ratio" else None
+    want, wst = emulated_place(bbox, active, table, area, mode, 99, 7, anchor, 0.5)
     got, gst = _gpu_place(bbox, active, table, area, mode, 99, 7, anchor, 0.5)
     assert np.array_equal(gst, wst) and np.array_equal(got, want)
     assert len(set(wst.tolist())) >= 1 and (wst > 0).mean() > 0.3

@@ -4,18 +4,18 @@ goal orientation samplers (rg_goal_orientations).
 
 The fixture tests/golden/reference_rearrange_goal.json.gz holds the reference's own results (tools/make_rearrange_goal_golden.py),
 the orientation draws from the same Philox counters as the kernel (tests/goal_rng.py).  The CPU tier runs the kernel's code
-on the emulation build (tests/emu_goal); the GPU tier runs it on the device.  Tolerances: positions 1e-12, angles 1e-9 rad,
+on the emulation build (tests/emu); the GPU tier runs it on the device.  Tolerances: positions 1e-12, angles 1e-9 rad,
 rotation distances 1e-7 (acos near 1 turns a last-bit difference of w into about 1e-8); decisions (the parallel quaternion,
 the greedy assignment, success flags) must agree wherever the reference's margin is wider than last-bit noise."""
 import ctypes
 import gzip
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import pyemu
 from goal_rng import GoalRotReplayRandomState
 from robogym_b200 import rearrange_goal as rg
 
@@ -23,22 +23,6 @@ ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_rearrange_goal.json.gz")
 ASSETS = os.path.join(ROOT, "robogym_b200", "assets")
 TABLE = np.array([1.3, 0.75, 0.2, 0.6075, 0.7655, 0.2])
-_emu = None
-
-
-def emu():
-    global _emu
-    if _emu is None:
-        here = os.path.join(ROOT, "tests", "emu_goal")
-        subprocess.check_call(["make", "-C", here, "-s"])
-        L = ctypes.CDLL(os.path.join(here, "_build", "librg_emu_goal.so"))
-        vp = ctypes.c_void_p
-        L.rge_goal.argtypes = [ctypes.POINTER(rg.GoalIn), vp, vp, ctypes.POINTER(rg.GoalOut)]
-        L.rge_goal_error.restype = ctypes.c_char_p
-        L.rge_goal_rot.argtypes = [ctypes.c_int, ctypes.c_int, vp, vp, ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32, vp, vp]
-        L.rge_parallel_quats.argtypes = [vp]
-        _emu = L
-    return _emu
 
 
 def _p(a):
@@ -85,9 +69,9 @@ class EmuGoal:
         ci.rot_dist_type = rg.ROT_DIST.get(self.mode, self.mode)
         ci.success_keys, ci.pos_threshold, ci.rot_threshold = _keys(self.threshold)
         ci.reward_per_object = self.reward_per_object
-        rc = emu().rge_goal(ctypes.byref(ci), _p(keep["mask"]), _p(self.prev), ctypes.byref(self.cout))
+        rc = pyemu.lib().rge_goal(ctypes.byref(ci), _p(keep["mask"]), _p(self.prev), ctypes.byref(self.cout))
         if rc != 0:
-            raise ValueError(emu().rge_goal_error().decode())
+            raise ValueError(pyemu.lib().rge_goal_error().decode())
         return {k: v.copy() for k, v in self.out.items()}
 
 
@@ -96,7 +80,7 @@ def emu_rot(base, active, seed, epoch, mode, mask=None, out=None):
     nenv, nobj = base.shape[:2]
     act = np.ascontiguousarray(np.broadcast_to(active, (nenv, nobj)), dtype=np.uint8)
     out = base.copy() if out is None else np.ascontiguousarray(out, dtype=np.float64)
-    emu().rge_goal_rot(nenv, nobj, _p(base), _p(act), rg.ROT_RANDOMIZE[mode], seed, epoch, _p(None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)), _p(out))
+    pyemu.lib().rge_goal_rot(nenv, nobj, _p(base), _p(act), rg.ROT_RANDOMIZE[mode], seed, epoch, _p(None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)), _p(out))
     return out
 
 
@@ -144,7 +128,7 @@ def check_case(c, got, want):
 # ---------------------------------------------------------------------------------------------- CPU
 def test_parallel_quaternion_tables_are_the_reference_tables(golden):
     out = np.zeros(112)
-    emu().rge_parallel_quats(_p(out))
+    pyemu.lib().rge_parallel_quats(_p(out))
     want = np.concatenate([np.ravel(golden["parallel_quats"]), np.ravel(golden["parallel_quats_180"])])
     assert np.array_equal(out, want) and np.array_equal(np.signbit(out), np.signbit(want))
 

@@ -3,18 +3,18 @@ placement-area masks, the contact flags and the simulation penalties of one env-
 
 The fixture tests/golden/reference_rearrange_obs.json.gz (tools/make_rearrange_obs_golden.py) holds the reference's own
 results on float32-rounded rows, with those rows, the goal and the index tables the reference's name lookups give.  The CPU tier
-runs the kernel's code on the emulation build (tests/emu_obs); the GPU tier runs it on the device.  Positions, velocities,
+runs the kernel's code on the emulation build (tests/emu); the GPU tier runs it on the device.  Positions, velocities,
 qpos, forces, contacts, masks, penalties and done must be bit-identical; angles and the qpos_goal quaternions agree within
 1e-14 (sin / cos / atan2, and the shim builds body_xmat with its own quat2mat)."""
 import ctypes
 import gzip
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import pyemu
 from robogym_b200 import rearrange_goal as rg
 from robogym_b200 import rearrange_obs as ro
 
@@ -22,19 +22,6 @@ ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_rearrange_obs.json.gz")
 ASSETS = os.path.join(ROOT, "robogym_b200", "assets")
 ANGLE_KEYS = ("obj_rot", "goal_obj_rot", "masked_obj_rot", "masked_goal_obj_rot")
-_emu = None
-
-
-def emu():
-    global _emu
-    if _emu is None:
-        here = os.path.join(ROOT, "tests", "emu_obs")
-        subprocess.check_call(["make", "-C", here, "-s"])
-        L = ctypes.CDLL(os.path.join(here, "_build", "librg_emu_obs.so"))
-        L.rge_obs.argtypes = [ctypes.POINTER(ro.ObsIn), ctypes.c_void_p, ctypes.POINTER(ro.ObsOut)]
-        L.rge_obs_error.restype = ctypes.c_char_p
-        _emu = L
-    return _emu
 
 
 @pytest.fixture(scope="module")
@@ -101,8 +88,8 @@ class EmuObs:
         for name in ("body_xpos", "body_xquat", "body_xvel", "qpos", "qvel", "ctrl", "sensordata", "contact", "ncon", "goal_pos", "goal_quat", "rel_pos",
                      "rel_rot", "achieved", "off_table", "group", "qpos_at_goal", "bbox_size", "colors", "boundary"):
             setattr(c, name, _p(k[name]))
-        if emu().rge_obs(ctypes.byref(c), _p(k["mask"]), ctypes.byref(self.cout)) != 0:
-            raise ValueError(emu().rge_obs_error().decode())
+        if pyemu.lib().rge_obs(ctypes.byref(c), _p(k["mask"]), ctypes.byref(self.cout)) != 0:
+            raise ValueError(pyemu.lib().rge_obs_error().decode())
         return self.out
 
 

@@ -26,9 +26,8 @@ def main():
     nenv = int(sys.argv[1]) if len(sys.argv) > 1 else 16
     steps = int(sys.argv[2]) if len(sys.argv) > 2 else 20
     build()
+    os.environ["RG_EMU_LIB"] = OUT
     import pyemu
-    pyemu._LIB = OUT
-    pyemu.subprocess = type("S", (), {"check_call": staticmethod(lambda *a, **k: 0)})
     from robogym_b200 import modelblob
     blob = open(os.path.join(ROOT, "robogym_b200", "assets", "dactyl_locked.rgm"), "rb").read()
     names = json.load(open(os.path.join(ROOT, "robogym_b200", "assets", "dactyl_locked.names.json")))
