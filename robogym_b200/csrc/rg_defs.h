@@ -164,7 +164,8 @@ enum { RG_WARN_CONTACT_FULL = 1, RG_WARN_ROWS_FULL = 2, RG_WARN_BAD_STATE = 4, R
        RG_WARN_PAIRS_FULL = 64 /* rg_batch_update_pairs: the environment's pair list overflowed its capacity (surplus dropped) */,
        RG_WARN_BAD_DATAID = 128 /* rg_batch_update_pairs: a geom_dataid value that is neither -1 nor a mesh id of a mesh geom (geom disabled) */ };
 
-/* Device view of the compiled model: fp32 / int32 copies of every rg_model_fields.h array. */
+/* Device view of the compiled model: fp32 / int32 copies of every rg_model_fields.h array, then the arrays the engine derives
+   (rg_derived_fields.h) and its derived scalars. */
 struct RgModel {
 #define RG_DIM(n) int n;
 #define RG_I(n, c) const int* n;
@@ -173,23 +174,13 @@ struct RgModel {
 #undef RG_DIM
 #undef RG_I
 #undef RG_F
-  const int* body_subtreesize; /* bodies are numbered depth-first: subtree(b) = [b, b+size) */
-  const int* dof_mrow;         /* [nv][3]: start of dof i's row in the tree-sparse mass matrix, dofs in its subtree, its depth */
-  const int* dof_lvl;          /* [2 nv + 2]: dof ids sorted by depth, then the start of every depth level (ndoflevel + 1 entries) */
-  const int* dof_xlvl;         /* the same lists restricted to the dofs that stay out of the constraint solver */
-  const int* dof_sidx;         /* [2 nv]: solver position of every dof (or -1), then the dof at every solver position */
-  const int* eqrow;            /* [neqrow]: equality id * 8 + row (weld: 6 rows, joint coupling: 1); row k is "virtual tendon" ntendon + k */
-  const float* mesh_scale;     /* [nmesh]: uniform scale of every hull (1 at load; model-wide or per-environment parameter) */
-  const float* geom_mesh_scale; /* [ngeom]: uniform scale of every mesh geom on top of its hull's mesh_scale (per-environment
-                                   parameter only), or nullptr = 1 everywhere */
-  const float* mesh_vert4;     /* [nmeshvert][4]: hull vertices padded to 16 bytes (one vector load each) */
-  const int* mesh_cell;        /* [nmesh][RG_NCELL][2]: (first entry in mesh_cand4, count) of every direction cell's support
-                                  candidates; count -1: scan the whole hull (rg_host_store_cells) */
-  const float* mesh_cand4;     /* [ncand][4]: candidate vertices x, y, z and the vertex id's int bits, ascending ids per cell;
-                                  right behind mesh_cell in the arena (the device finds it there: rg_hull_cands) */
+#define RG_DS(n, T, c) const T* n;
+#define RG_DE(n, T, c) const T* n;
+#define RG_DG(n, T, c) const T* n;
+#include "rg_derived_fields.h"
   int ncand_cap;               /* entries mesh_cand4 has room for (rebuilt lists must fit in the arena allocated at load) */
-  const unsigned short* pair_packed; /* [npair] geom1 | geom2 << 8 when ngeom <= 256 (staged in shared memory), else nullptr;
-                                        a view with pair_geom2 == nullptr streams an environment's own list instead (rg_pair) */
+#define RG_DSO(n, T, c, when) const T* n;
+#include "rg_derived_fields.h"
   float origin[3];             /* world translation applied at load so coordinates stay small in fp32 */
   int small_bytes;             /* leading part of the arena that is staged into shared memory */
   int nM;                      /* entries of the tree-sparse mass matrix: sum over dofs of (depth + 1) */
@@ -239,18 +230,16 @@ struct RgModelDev {
 #undef RG_F
 #undef RG_IB
 #undef RG_FB
-  RgArr<int> body_subtreesize;
-  RgArr<int> dof_mrow;
-  RgArr<int> dof_lvl;
-  RgArr<int> dof_xlvl;
-  RgArr<int> dof_sidx;
-  RgArr<int> eqrow;
-  RgArr<float> mesh_scale;
-  RgArr<float> geom_mesh_scale;   /* off < 0 while no per-environment row is bound: never staged, so it costs no shared memory */
-  RgArr<unsigned short> pair_packed;
+  /* a per-environment array's offset is < 0 while no row is bound: it is never staged, so it costs no shared memory */
+#define RG_DS(n, T, c) RgArr<T> n;
+#define RG_DE(n, T, c) RgArr<T> n;
+#include "rg_derived_fields.h"
+#define RG_DSO(n, T, c, when) RgArr<T> n;
+#include "rg_derived_fields.h"
   int has_pairs;
-  const float* mesh_vert4;
-  const int* mesh_cell;        /* the candidate entries follow the table (rg_hull_cands) */
+#define RG_DG(n, T, c) const T* n;
+#define RG_DGH(n, T, c)
+#include "rg_derived_fields.h"
   float origin[3];
   int small_bytes;
   int nM;

@@ -104,19 +104,17 @@ __global__ void __launch_bounds__(RG_MAX_WARPS * 32, 1) rg_step_kernel(const __g
 #undef RG_F
 #undef RG_IB
 #undef RG_FB
-    RG_SETOFF(body_subtreesize)
-    RG_SETOFF(dof_mrow)
-    RG_SETOFF(dof_lvl)
-    RG_SETOFF(dof_xlvl)
-    RG_SETOFF(dof_sidx)
-    RG_SETOFF(eqrow)
-    RG_SETOFF(mesh_scale)
-    RG_SETPTR(mesh_vert4)
-    RG_SETPTR(mesh_cell)
+#define RG_DS(n, T, c) RG_SETOFF(n)
+#define RG_DG(n, T, c) RG_SETPTR(n)
+#define RG_DGH(n, T, c)
+#include "rg_derived_fields.h"
     if (lane == 0) {
       sm->has_pairs = args.m.pair_packed != nullptr;
-      sm->geom_mesh_scale.off = -1;   /* unbound: every factor 1 (a bound row overwrites the offset in the warp's own view) */
-      sm->pair_packed.off = args.m.pair_packed ? model_bytes + (int)((const char*)args.m.pair_packed - abase) : 0;
+      /* per-environment arrays are unbound: every factor 1 (a bound row overwrites the offset in the warp's own view) */
+#define RG_DE(n, T, c) sm->n.off = -1;
+#include "rg_derived_fields.h"
+#define RG_DSO(n, T, c, when) sm->n.off = args.m.n ? model_bytes + (int)((const char*)args.m.n - abase) : 0;
+#include "rg_derived_fields.h"
       sm->origin[0] = args.m.origin[0]; sm->origin[1] = args.m.origin[1]; sm->origin[2] = args.m.origin[2];
       sm->small_bytes = small_bytes;
       sm->nM = args.m.nM;
@@ -349,8 +347,6 @@ struct rg_model {
   char* d_arena = nullptr;
   int device = 0;
   RgLayout L;
-  std::vector<std::string> names;
-  std::vector<size_t> src_counts;
   bool disabled_parts = false;   /* some mesh geom has geom_dataid -1: its batches always stream per-environment pair lists */
 };
 struct rg_batch {
@@ -389,19 +385,32 @@ static void rg_wire_device_view(rg_model* mm) {
 #undef RG_DIM
 #undef RG_I
 #undef RG_F
-  RG_DEVPTR(body_subtreesize)
-  RG_DEVPTR(dof_mrow)
-  RG_DEVPTR(dof_lvl)
-  RG_DEVPTR(dof_xlvl)
-  RG_DEVPTR(dof_sidx)
-  RG_DEVPTR(eqrow)
-  RG_DEVPTR(mesh_scale)
-  RG_DEVPTR(mesh_vert4)
-  RG_DEVPTR(mesh_cell)
-  RG_DEVPTR(mesh_cand4)
-  if (mm->hm.view.pair_packed) RG_DEVPTR(pair_packed)
+#define RG_DS(n, T, c) RG_DEVPTR(n)
+#define RG_DSO(n, T, c, when) if (mm->hm.view.n) RG_DEVPTR(n)
+#define RG_DG(n, T, c) RG_DEVPTR(n)
+#include "rg_derived_fields.h"
 #undef RG_DEVPTR
 }
+
+/* byte offset in RgModelDev of every array that lives in shared memory, which a warp's own view may point at a per-environment
+   row instead (rg_batch_bind_param) */
+static const struct { const char* name; int off; } rg_dev_arrays[] = {
+#define RG_DIM(n)
+#define RG_I(n, c) {#n, (int)offsetof(RgModelDev, n)},
+#define RG_F(n, c) {#n, (int)offsetof(RgModelDev, n)},
+#define RG_IB(n, c)
+#define RG_FB(n, c)
+#include "../../include/rg_model_fields.h"
+#undef RG_DIM
+#undef RG_I
+#undef RG_F
+#undef RG_IB
+#undef RG_FB
+#define RG_DS(n, T, c) {#n, (int)offsetof(RgModelDev, n)},
+#define RG_DSO(n, T, c, when) {#n, (int)offsetof(RgModelDev, n)},
+#define RG_DE(n, T, c) {#n, (int)offsetof(RgModelDev, n)},
+#include "rg_derived_fields.h"
+};
 
 extern "C" {
 
@@ -470,36 +479,20 @@ int rg_model_set_field(rg_model* mm, const char* name, const void* data, size_t 
 int rg_model_set_field_async(rg_model* mm, const char* name, const void* data, size_t count, void* stream) {
   if (!mm || !name || !data) return rg_fail(-1, "rg_model_set_field: null argument");
   RgModel& m = mm->hm.view;
-#define RG_DIM(n) const int n = m.n; (void)n;
-#define RG_I(n, c)
-#define RG_F(n, c)
-#include "../../include/rg_model_fields.h"
-#undef RG_DIM
-#undef RG_I
-#undef RG_F
-  void* hptr = nullptr;
-  size_t n = 0;
-  int isint = 0;
-#define RG_DIM(n)
-#define RG_I(f, c) if (!strcmp(name, #f)) { hptr = (void*)m.f; n = (size_t)(c); isint = 1; }
-#define RG_F(f, c) if (!strcmp(name, #f)) { hptr = (void*)m.f; n = (size_t)(c); isint = 0; }
-#include "../../include/rg_model_fields.h"
-#undef RG_DIM
-#undef RG_I
-#undef RG_F
   if (!strcmp(name, "geom_mesh_scale"))
     return rg_fail(-1, "rg_model_set_field: geom_mesh_scale exists per environment only (rg_batch_bind_param); scale hulls model-wide with mesh_scale");
-  const bool is_scale = !strcmp(name, "mesh_scale");   /* derived array of the engine, not a blob field */
-  if (is_scale) { hptr = (void*)m.mesh_scale; n = (size_t)m.nmesh; }
-  if (!hptr) return rg_fail(-1, std::string("rg_model_set_field: unknown field ") + name);
+  const bool is_scale = !strcmp(name, "mesh_scale");   /* the one derived array of the engine that is a model parameter */
+  RgHostField f;
+  if (!rg_host_field(m, name, f) || (f.derived && !is_scale)) return rg_fail(-1, std::string("rg_model_set_field: unknown field ") + name);
+  const size_t n = f.count;
   if (n != count) return rg_fail(-1, std::string("rg_model_set_field: size mismatch for ") + name);
   if (is_scale)
     for (size_t i = 0; i < n; i++)
       if (!(((const double*)data)[i] > 0.0) || !isfinite(((const double*)data)[i])) return rg_fail(-1, "rg_model_set_field: mesh_scale must be finite and positive");
-  if (isint) memcpy(hptr, data, 4 * n);
+  if (f.isint) memcpy(f.p, data, 4 * n);
   else {
     const double* s = (const double*)data;
-    float* d = (float*)hptr;
+    float* d = (float*)f.p;
     for (size_t i = 0; i < n; i++) d[i] = (float)s[i];
     if (!strcmp(name, "body_pos")) /* keep the fp32 world shift */
       for (int b = 1; b < m.nbody; b++)
@@ -507,17 +500,20 @@ int rg_model_set_field_async(rg_model* mm, const char* name, const void* data, s
     if (!strcmp(name, "geom_pos")) for (int g = 0; g < m.ngeom; g++) if (m.geom_bodyid[g] == 0) for (int a = 0; a < 3; a++) d[3 * g + a] -= m.origin[a];
     if (!strcmp(name, "site_pos")) for (int k = 0; k < m.nsite; k++) if (m.site_bodyid[k] == 0) for (int a = 0; a < 3; a++) d[3 * k + a] -= m.origin[a];
   }
-  const size_t off = (const char*)hptr - mm->hm.arena.data();
   RG_CUDA(cudaSetDevice(mm->device));
   /* stream-ordered: launches already queued on `stream` still see the old values, later ones the new; the host copy is
      pageable, so the runtime stages it before returning and `data` / the host arena may change right away */
-  RG_CUDA(cudaMemcpyAsync(mm->d_arena + off, hptr, 4 * n, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  auto upload = [&](const char* array) {
+    RgHostField u;
+    rg_host_field(m, array, u);
+    return cudaMemcpyAsync(mm->d_arena + ((const char*)u.p - mm->hm.arena.data()), u.p, 4 * u.count, cudaMemcpyHostToDevice, (cudaStream_t)stream);
+  };
+  RG_CUDA(upload(name));
   if (!strcmp(name, "mesh_vert")) {
     /* what the narrow phase derives from the hulls follows them: the float4-padded copy it scans, and the geom-frame box of
        every mesh geom that the OBB cull tests (the vertex bounding box, as the model compiler computes it) */
     rg_host_pad_verts(m);
-    const size_t off4 = (const char*)m.mesh_vert4 - mm->hm.arena.data();
-    RG_CUDA(cudaMemcpyAsync(mm->d_arena + off4, m.mesh_vert4, 16 * (size_t)m.nmeshvert, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    RG_CUDA(upload("mesh_vert4"));
     const double* v = (const double*)data;
     float* aabb = (float*)m.geom_aabb;
     for (int g = 0; g < m.ngeom; g++) {
@@ -532,8 +528,7 @@ int rg_model_set_field_async(rg_model* mm, const char* name, const void* data, s
         aabb[6 * g + 3 + k] = (float)(0.5 * (hi - lo));
       }
     }
-    const size_t offb = (const char*)m.geom_aabb - mm->hm.arena.data();
-    RG_CUDA(cudaMemcpyAsync(mm->d_arena + offb, m.geom_aabb, 24 * (size_t)m.ngeom, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    RG_CUDA(upload("geom_aabb"));
   }
   const bool vert = !strcmp(name, "mesh_vert"), layout = !strcmp(name, "mesh_vertadr") || !strcmp(name, "mesh_vertnum");
   if (vert || layout) {
@@ -544,9 +539,8 @@ int rg_model_set_field_async(rg_model* mm, const char* name, const void* data, s
       m.ncand_cap = 0;
       rg_host_store_cells(m, std::vector<int>(2 * (size_t)m.nmesh * RG_NCELL, -1), std::vector<int>());
     }
-    const size_t offc = (const char*)m.mesh_cell - mm->hm.arena.data(), offe = (const char*)m.mesh_cand4 - mm->hm.arena.data();
-    RG_CUDA(cudaMemcpyAsync(mm->d_arena + offc, m.mesh_cell, 8 * (size_t)m.nmesh * RG_NCELL, cudaMemcpyHostToDevice, (cudaStream_t)stream));
-    if (m.ncand_cap > 0) RG_CUDA(cudaMemcpyAsync(mm->d_arena + offe, m.mesh_cand4, 16 * (size_t)m.ncand_cap, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    RG_CUDA(upload("mesh_cell"));
+    if (m.ncand_cap > 0) RG_CUDA(upload("mesh_cand4"));
   }
   return 0;
 }
@@ -688,31 +682,14 @@ int rg_model_origin(const rg_model* m, float origin[3]) {
 int rg_batch_bind_param(rg_batch* b, const char* name, void* p) {
   if (!b || !name) return rg_fail(-1, "rg_batch_bind_param: null argument");
   const RgModel& m = b->model->hm.view;
-#define RG_DIM(n) const int n = m.n; (void)n;
-#define RG_I(n, c)
-#define RG_F(n, c)
-#include "../../include/rg_model_fields.h"
-#undef RG_DIM
-#undef RG_I
-#undef RG_F
-  int off = -1, cnt = 0;
-#define RG_DIM(n)
-#define RG_I(f, c)
-#define RG_IB(f, c)
-#define RG_FB(f, c)
-#define RG_F(f, c) if (!strcmp(name, #f)) { off = (int)offsetof(RgModelDev, f); cnt = (int)(c); }
-#include "../../include/rg_model_fields.h"
-#undef RG_DIM
-#undef RG_I
-#undef RG_F
-#undef RG_IB
-#undef RG_FB
-  if (!strcmp(name, "mesh_scale")) { off = (int)offsetof(RgModelDev, mesh_scale); cnt = m.nmesh; }
-  if (!strcmp(name, "geom_mesh_scale")) { off = (int)offsetof(RgModelDev, geom_mesh_scale); cnt = ngeom; }
+  int off = -1;
+  for (const auto& a : rg_dev_arrays) if (!strcmp(name, a.name)) off = a.off;
   const bool dataid = !strcmp(name, "geom_dataid");   /* the one int array: per-environment mesh draws (rg_batch_update_pairs) */
-  if (dataid) { off = (int)offsetof(RgModelDev, geom_dataid); cnt = ngeom; }
-  if (off < 0) return rg_fail(-1, std::string("rg_batch_bind_param: not a (small) float model array: ") + name);
-  if (dataid && ngeom > 65536) return rg_fail(-1, "rg_batch_bind_param: geom_dataid per environment needs ngeom <= 65536 (16-bit ids in the pair lists)");
+  RgHostField f;
+  if (off < 0 || !rg_host_field(m, name, f) || (f.isint && !dataid))
+    return rg_fail(-1, std::string("rg_batch_bind_param: not a (small) float model array: ") + name);
+  const int cnt = (int)f.count;
+  if (dataid && m.ngeom > 65536) return rg_fail(-1, "rg_batch_bind_param: geom_dataid per environment needs ngeom <= 65536 (16-bit ids in the pair lists)");
   int slot = -1;
   for (int i = 0; i < b->nover; i++) if (b->over_name[i] == name) slot = i;
   if (!p) {

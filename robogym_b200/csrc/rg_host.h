@@ -10,6 +10,7 @@
 
 #include <map>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "rg_defs.h"
@@ -17,12 +18,52 @@
 struct RgHostModel {
   std::vector<char> arena;
   RgModel view;                 /* pointers into `arena` (host) */
-  std::vector<size_t> offsets;  /* byte offset of every RgModel pointer field, in struct order */
   size_t small_bytes = 0;
   std::map<std::string, std::vector<std::string>> names;   /* objtype -> names ("" = unnamed), from the blob's RGNAMES1 section */
 };
 
+/* the blob's arrays where they lie in the blob: int32 and fp64 */
+struct RgBlob {
+#define RG_DIM(n)
+#define RG_I(n, c) const int* n;
+#define RG_F(n, c) const double* n;
+#include "../../include/rg_model_fields.h"
+#undef RG_DIM
+#undef RG_I
+#undef RG_F
+};
+
 static inline size_t rg_align16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+/* A model array by name: one of the blob's (include/rg_model_fields.h) or one the engine derives (rg_derived_fields.h), with its
+   element count.  The pointer is the view's: nullptr for an array the view does not hold (a per-environment one, or
+   pair_packed when the pairs are not packed). */
+struct RgHostField { void* p; size_t count; bool isint, derived; };
+static inline bool rg_host_field(const RgModel& m, const char* name, RgHostField& f) {
+#define RG_DIM(n) const int n = m.n; (void)n;
+#define RG_I(n, c)
+#define RG_F(n, c)
+#include "../../include/rg_model_fields.h"
+#undef RG_DIM
+#undef RG_I
+#undef RG_F
+  const int ncand_cap = m.ncand_cap; (void)ncand_cap;
+#define RG_FIELD(n, T, c, d) if (!strcmp(name, #n)) { f = {(void*)m.n, (size_t)(c), std::is_integral<T>::value, d}; return true; }
+#define RG_DIM(n)
+#define RG_I(n, c) RG_FIELD(n, int, c, false)
+#define RG_F(n, c) RG_FIELD(n, float, c, false)
+#include "../../include/rg_model_fields.h"
+#undef RG_DIM
+#undef RG_I
+#undef RG_F
+#define RG_DS(n, T, c) RG_FIELD(n, T, c, true)
+#define RG_DSO(n, T, c, when) RG_FIELD(n, T, (when) ? (c) : 0, true)
+#define RG_DE(n, T, c) RG_FIELD(n, T, c, true)
+#define RG_DG(n, T, c) RG_FIELD(n, T, c, true)
+#include "rg_derived_fields.h"
+#undef RG_FIELD
+  return false;
+}
 
 /* (re)build the float4-padded hull vertices the narrow phase reads from mesh_vert (at load, and after mesh_vert was edited) */
 static inline void rg_host_pad_verts(RgModel& m) {
@@ -165,23 +206,21 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
 #undef RG_DIM
 #undef RG_I
 #undef RG_F
-  /* pass 1: sizes */
-  size_t src = 12 + 4 * (size_t)ndim, dst = 0;
-  std::vector<size_t> srcoff, dstoff, counts;
-  std::vector<int> isint;
-  std::vector<std::string> names;
+  /* where the blob's arrays lie: each on an 8-byte boundary */
+  RgBlob src;
+  size_t at = 12 + 4 * (size_t)ndim;
 #define RG_DIM(n)
-#define RG_I(n, c) src = (src + 7) & ~(size_t)7; srcoff.push_back(src); src += 4 * (size_t)(c); dst = rg_align16(dst); dstoff.push_back(dst); dst += 4 * (size_t)(c); counts.push_back((size_t)(c)); isint.push_back(1); names.push_back(#n);
-#define RG_F(n, c) src = (src + 7) & ~(size_t)7; srcoff.push_back(src); src += 8 * (size_t)(c); dst = rg_align16(dst); dstoff.push_back(dst); dst += 4 * (size_t)(c); counts.push_back((size_t)(c)); isint.push_back(0); names.push_back(#n);
+#define RG_I(n, c) at = (at + 7) & ~(size_t)7; src.n = (const int*)(p + at); at += 4 * (size_t)(c);
+#define RG_F(n, c) at = (at + 7) & ~(size_t)7; src.n = (const double*)(p + at); at += 8 * (size_t)(c);
 #include "../../include/rg_model_fields.h"
 #undef RG_DIM
 #undef RG_I
 #undef RG_F
-  if (src > len) { err = "model blob truncated"; return false; }
+  if (at > len) { err = "model blob truncated"; return false; }
   /* optional name tables behind the arrays (mjModel.*_name2id): RGNAMES1, ntypes, then type\0 count name\0 ... */
   hm.names.clear();
   {
-    size_t q = (src + 7) & ~(size_t)7;
+    size_t q = (at + 7) & ~(size_t)7;
     if (q + 12 <= len && !memcmp(p + q, "RGNAMES1", 8)) {
       int nt;
       memcpy(&nt, p + q + 8, 4);
@@ -208,69 +247,67 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
      layout, which sizes their room: what they take now plus a quarter for later mesh_vert edits (rg_host_store_cells) */
   std::vector<int> cell_table, cell_ids;
   {
-    size_t iv = 0, ia = 0, in = 0;
-    for (size_t i = 0; i < names.size(); i++) {
-      if (names[i] == "mesh_vert") iv = i;
-      else if (names[i] == "mesh_vertadr") ia = i;
-      else if (names[i] == "mesh_vertnum") in = i;
-    }
-    const int* va = (const int*)(p + srcoff[ia]); const int* vn = (const int*)(p + srcoff[in]);
+    const int* va = src.mesh_vertadr; const int* vn = src.mesh_vertnum;
     for (int h = 0; h < m.nmesh; h++)
       if (va[h] < 0 || vn[h] < 0 || va[h] > m.nmeshvert - vn[h]) { err = "mesh_vertadr / mesh_vertnum out of range"; return false; }
-    const double* sv = (const double*)(p + srcoff[iv]);
     std::vector<float> v4(4 * (size_t)m.nmeshvert, 0.0f);
-    for (size_t k = 0; k < (size_t)m.nmeshvert; k++) for (int a = 0; a < 3; a++) v4[4 * k + a] = (float)sv[3 * k + a];
+    for (size_t k = 0; k < (size_t)m.nmeshvert; k++) for (int a = 0; a < 3; a++) v4[4 * k + a] = (float)src.mesh_vert[3 * k + a];
     rg_host_cells(v4.data(), va, vn, m.nmesh, cell_table, cell_ids);
   }
   const size_t ncand_cap = cell_ids.size() + cell_ids.size() / 4;
   if (ncand_cap > (size_t)0x7fffffff) { err = "hull support lists too large"; return false; }
-  /* derived arrays appended to the small section would disturb the order; put them right after the blob fields
-     but account for them in small_bytes by placing them BEFORE the first big field. */
-  size_t first_big = names.size();
-  for (size_t i = 0; i < names.size(); i++) if (names[i] == "mesh_vert") { first_big = i; break; }
-  /* re-run the destination layout: small fields, derived, big fields */
-  dst = 0;
-  for (size_t i = 0; i < first_big; i++) { dst = rg_align16(dst); dstoff[i] = dst; dst += 4 * counts[i]; }
-  dst = rg_align16(dst); const size_t off_subtree = dst; dst += 4 * (size_t)m.nbody;
-  dst = rg_align16(dst); const size_t off_mrow = dst; dst += 12 * (size_t)m.nv;
-  dst = rg_align16(dst); const size_t off_dlvl = dst; dst += 4 * (2 * (size_t)m.nv + 2);
-  dst = rg_align16(dst); const size_t off_xlvl = dst; dst += 4 * (2 * (size_t)m.nv + 2);
-  dst = rg_align16(dst); const size_t off_sidx = dst; dst += 4 * (2 * (size_t)m.nv);
-  dst = rg_align16(dst); const size_t off_eqrow = dst; dst += 4 * (6 * (size_t)m.neq + 1);
-  dst = rg_align16(dst); const size_t off_pairs = dst; if (m.ngeom <= 256) dst += 2 * (size_t)m.npair;
-  dst = rg_align16(dst); const size_t off_mscale = dst; dst += 4 * (size_t)m.nmesh;
-  dst = rg_align16(dst);
-  hm.small_bytes = dst;
-  for (size_t i = first_big; i < names.size(); i++) { dst = rg_align16(dst); dstoff[i] = dst; dst += 4 * counts[i]; }
-  dst = rg_align16(dst); const size_t off_v4 = dst; dst += 16 * (size_t)m.nmeshvert;
-  dst = rg_align16(dst); const size_t off_cell = dst; dst += 8 * (size_t)m.nmesh * RG_NCELL;
-  const size_t off_cand = dst; dst += 16 * ncand_cap;   /* right behind the table (8 * RG_NCELL is a multiple of 16): rg_hull_cands */
-  dst = rg_align16(dst);
-  hm.arena.assign(dst, 0);
-  char* base = hm.arena.data();
-  for (size_t i = 0; i < names.size(); i++) {
-    if (isint[i]) memcpy(base + dstoff[i], p + srcoff[i], 4 * counts[i]);
-    else {
-      const double* s = (const double*)(p + srcoff[i]);
-      float* d = (float*)(base + dstoff[i]);
-      for (size_t q = 0; q < counts[i]; q++) d[q] = (float)s[q];
-    }
-  }
-  /* wire the view */
-  size_t idx = 0;
-  hm.offsets.clear();
+  /* The arena, every array 16-byte aligned: the blob's small arrays and the derived staged ones (the leading small_bytes, which
+     every CTA stages into shared memory), then the blob's big arrays and the derived global ones.  Walked once to size it, then
+     once more to point the view's arrays into it and copy the blob's arrays there (fp64 -> fp32). */
+  static_assert(8 * RG_NCELL % 16 == 0, "mesh_cand4 must start right behind mesh_cell (rg_hull_cands)");
+  char* base = nullptr;
+  size_t dst = 0;
+  auto put = [&](auto& ptr, size_t count, bool present) {
+    dst = rg_align16(dst);
+    if (base) ptr = present ? (std::remove_reference_t<decltype(ptr)>)(base + dst) : nullptr;
+    if (present) dst += sizeof(*ptr) * count;
+  };
+  auto put_i = [&](const int*& ptr, const int* s, size_t count) { put(ptr, count, true); if (base) memcpy((void*)ptr, s, 4 * count); };
+  auto put_f = [&](const float*& ptr, const double* s, size_t count) { put(ptr, count, true); if (base) for (size_t q = 0; q < count; q++) ((float*)ptr)[q] = (float)s[q]; };
+  auto layout = [&]() {
+    dst = 0;
 #define RG_DIM(n)
-#define RG_I(n, c) m.n = (const int*)(base + dstoff[idx]); hm.offsets.push_back(dstoff[idx]); idx++;
-#define RG_F(n, c) m.n = (const float*)(base + dstoff[idx]); hm.offsets.push_back(dstoff[idx]); idx++;
+#define RG_I(n, c) put_i(m.n, src.n, (size_t)(c));
+#define RG_F(n, c) put_f(m.n, src.n, (size_t)(c));
+#define RG_IB(n, c)
+#define RG_FB(n, c)
+#include "../../include/rg_model_fields.h"
+#undef RG_IB
+#undef RG_FB
+#define RG_DS(n, T, c) put(m.n, (size_t)(c), true);
+#define RG_DSO(n, T, c, when) put(m.n, (size_t)(c), (when));
+#include "rg_derived_fields.h"
+    hm.small_bytes = dst = rg_align16(dst);
+#undef RG_I
+#undef RG_F
+#define RG_I(n, c)
+#define RG_F(n, c)
+#define RG_IB(n, c) put_i(m.n, src.n, (size_t)(c));
+#define RG_FB(n, c) put_f(m.n, src.n, (size_t)(c));
 #include "../../include/rg_model_fields.h"
 #undef RG_DIM
 #undef RG_I
 #undef RG_F
+#undef RG_IB
+#undef RG_FB
+#define RG_DG(n, T, c) put(m.n, (size_t)(c), true);
+#include "rg_derived_fields.h"
+    dst = rg_align16(dst);
+  };
+  layout();
+  hm.arena.assign(dst, 0);
+  base = hm.arena.data();
+  layout();
   /* rows of the equality constraints (weld: 3 position + 3 orientation rows, joint coupling: 1) -- of all of them: eq_active is
      read at run time, robogym switches welds off and on (robogym/envs/rearrange/common/base.py:452).  Constraint types the
      compiler can describe but this engine does not simulate are refused instead of stepping wrong physics */
   {
-    int* eqrow = (int*)(base + off_eqrow);
+    int* eqrow = (int*)m.eqrow;
     int n = 0;
     for (int e = 0; e < m.neq; e++) {
       if (m.eq_type[e] == RG_EQ_WELD) {
@@ -283,15 +320,14 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
       else { err = "equality constraint type other than weld / joint: not supported by this engine"; return false; }
     }
     m.neqrow = n;
-    m.eqrow = eqrow;
   }
   /* mujoco-py's second user controller (actuator_user[0] = 1: the cascaded-PI law of the UR16e's default joint calibration,
      robogym/assets/xmls/robot/ur16e/jointspec/calibrations/cascaded_pi/joint_actuations.xml:4) keeps 6 floats of state per actuator */
   m.pidw = 3;
   for (int i = 0; i < m.nu; i++)
     if (m.actuator_user0[i] == 1.0f && m.actuator_biastype[i] == RG_BIAS_USER) m.pidw = 6;
-  int* subtree = (int*)(base + off_subtree);
-  int* mrow = (int*)(base + off_mrow);
+  int* subtree = (int*)m.body_subtreesize;
+  int* mrow = (int*)m.dof_mrow;
   for (int b = 0; b < m.nbody; b++) subtree[b] = 1;
   for (int b = m.nbody - 1; b > 0; b--) subtree[m.body_parentid[b]] += subtree[b];
   /* tree-sparse mass matrix (MuJoCo's qM layout): row i holds M(i,i), M(i,parent(i)), M(i,parent(parent(i))), ... */
@@ -313,7 +349,7 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
     m.nM = nM;
     /* dofs sorted by depth (stable): dlvl[0..nv) = dof ids, dlvl[nv + l] = start of level l; the tree-sparse
        factorisation walks these levels leaves-first, the back substitution roots-first */
-    int* dlvl = (int*)(base + off_dlvl);
+    int* dlvl = (int*)m.dof_lvl;
     int maxd = 0;
     for (int d = 0; d < m.nv; d++) if (mrow[3 * d + 2] > maxd) maxd = mrow[3 * d + 2];
     int pos = 0;
@@ -323,7 +359,6 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
     }
     dlvl[m.nv + maxd + 1] = pos;
     m.ndoflevel = m.nv > 0 ? maxd + 1 : 0;
-    m.dof_lvl = dlvl;
     /* Kinematic trees that no constraint row can ever touch (no friction loss, no limited joint, no tendon, no geom in a
        collision pair -- e.g. the collision-free target cube of the dactyl scenes, robogym/envs/dactyl/locked.py:89-96) stay
        out of the constraint solver: their acceleration is M^-1 qfrc_smooth exactly (tree-sparse solve), and the dense
@@ -344,69 +379,41 @@ static inline bool rg_host_load(const void* blob, size_t len, RgHostModel& hm, s
       if (m.eq_type[e] == RG_EQ_WELD) { mark_body(m.eq_obj1id[e]); mark_body(m.eq_obj2id[e]); }
       else { mark_body(m.jnt_bodyid[m.eq_obj1id[e]]); if (m.eq_obj2id[e] >= 0) mark_body(m.jnt_bodyid[m.eq_obj2id[e]]); }
     }
-    int* sidx = (int*)(base + off_sidx);
+    int* sidx = (int*)m.dof_sidx;
     int ns = 0;
     for (int d = m.nv - 1; d >= 0; d--) {
       if (tree_con[m.body_rootid[m.dof_bodyid[d]]]) { sidx[d] = ns; sidx[m.nv + ns] = d; ns++; }
       else sidx[d] = -1;
     }
     m.ns = ns;
-    m.dof_sidx = sidx;
-    int* xlvl = (int*)(base + off_xlvl);
+    int* xlvl = (int*)m.dof_xlvl;
     pos = 0;
     for (int l = 0; l <= maxd; l++) {
       xlvl[m.nv + l] = pos;
       for (int d = 0; d < m.nv; d++) if (mrow[3 * d + 2] == l && sidx[d] < 0) xlvl[pos++] = d;
     }
     xlvl[m.nv + maxd + 1] = pos;
-    m.dof_xlvl = xlvl;
   }
   /* depth-first numbering check: every body's parent must precede it and subtrees must be contiguous */
   for (int b = 1; b < m.nbody; b++) {
     const int par = m.body_parentid[b];
     if (par >= b || b >= par + subtree[par]) { err = "bodies are not numbered depth-first"; return false; }
   }
-  m.body_subtreesize = subtree;
-  m.dof_mrow = mrow;
-  hm.offsets.push_back(off_subtree);
-  hm.offsets.push_back(off_mrow);
-  hm.offsets.push_back(off_dlvl);
-  hm.offsets.push_back(off_xlvl);
-  hm.offsets.push_back(off_sidx);
-  hm.offsets.push_back(off_eqrow);
   /* uniform hull scale: the narrow phase's support point of a mesh is mesh_scale * (arg-max vertex of the unscaled hull) */
-  float* mscale = (float*)(base + off_mscale);
-  for (int k = 0; k < m.nmesh; k++) mscale[k] = 1.0f;
-  m.mesh_scale = mscale;
-  m.geom_mesh_scale = nullptr;   /* per-environment only (rg_batch_bind_param): never part of the arena */
-  hm.offsets.push_back(off_mscale);
+  for (int k = 0; k < m.nmesh; k++) ((float*)m.mesh_scale)[k] = 1.0f;
   /* hull vertices padded to float4: the narrow phase scans a hull's vertices with one 16-byte load each */
-  float* v4 = (float*)(base + off_v4);
-  m.mesh_vert4 = v4;
   rg_host_pad_verts(m);
-  m.pair_packed = nullptr;
-  if (m.ngeom <= 256) {
-    unsigned short* pk = (unsigned short*)(base + off_pairs);
+  if (m.pair_packed) {   /* ngeom <= 256 */
+    unsigned short* pk = (unsigned short*)m.pair_packed;
     for (int k = 0; k < m.npair; k++) pk[k] = (unsigned short)(m.pair_geom1[k] | (m.pair_geom2[k] << 8));
-    m.pair_packed = pk;
   }
-  hm.offsets.push_back(off_v4);
   /* the hulls' support candidate lists (global memory, behind the staged section: shared memory per CTA is unchanged) */
-  m.mesh_cell = (const int*)(base + off_cell);
-  m.mesh_cand4 = (const float*)(base + off_cand);
   m.ncand_cap = (int)ncand_cap;
   rg_host_store_cells(m, cell_table, cell_ids);
-  hm.offsets.push_back(off_cell);
-  hm.offsets.push_back(off_cand);
   /* fp32 conditioning: translate the world so the scene sits near the origin */
   double o[3] = {0, 0, 0};
   int cnt = 0;
-  const double* bp = nullptr;
-  {
-    size_t i = 0;
-    for (; i < names.size(); i++) if (names[i] == "body_pos") break;
-    bp = (const double*)(p + srcoff[i]);
-  }
+  const double* bp = src.body_pos;
   for (int b = 1; b < m.nbody; b++) if (m.body_parentid[b] == 0) { for (int a = 0; a < 3; a++) o[a] += bp[3 * b + a]; cnt++; }
   for (int a = 0; a < 3; a++) m.origin[a] = cnt ? (float)(o[a] / cnt) : 0.0f;
   float* body_pos = (float*)m.body_pos;

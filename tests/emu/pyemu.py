@@ -38,9 +38,7 @@ def lib():
         L.rge_set_sensordata.argtypes = [vp, vp]
         L.rge_set_mocap.argtypes = [vp, vp, vp]
         L.rge_step.argtypes = [vp, ci] + [vp] * 18 + [ci, ci]
-        # a handle's model view: mesh scale, pair lists, geom scale
-        L.rge_mesh_scale.restype = vp
-        L.rge_mesh_scale.argtypes = [vp, pi]
+        # a handle's model view: pair lists, geom scale
         L.rge_pairs.argtypes = [vp, vp, vp, ci, pi]
         L.rge_use_pairs.argtypes = [vp, vp, ci]
         L.rge_use_geom_scale.argtypes = [vp, vp]
@@ -121,12 +119,6 @@ class EmuBatch:
         p = lib().rge_model_field(self.h, name.encode(), ctypes.byref(n))
         ct = ctypes.c_int32 if dtype == np.int32 else ctypes.c_float
         return np.frombuffer((ct * n.value).from_address(p), dtype=dtype)
-
-    def mesh_scale(self):
-        """writable float32 view of the model's [nmesh] mesh_scale (engine-derived, so model_field does not serve it)"""
-        n = ctypes.c_int()
-        p = lib().rge_mesh_scale(self.h, ctypes.byref(n))
-        return np.frombuffer((ctypes.c_float * n.value).from_address(p), dtype=np.float32)
 
     def use_pairs(self, pairs, n):
         """step the first n pairs of `pairs` (packed g1 | g2 << 16) instead of the model's static list, as the engine does for an

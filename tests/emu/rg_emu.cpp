@@ -76,25 +76,12 @@ void rge_destroy(void* hv) { delete (RgeHandle*)hv; }
 int rge_dbg_size(void* hv) { return rg_dbg_size(((RgeHandle*)hv)->hm.view, ((RgeHandle*)hv)->L.ncon); }
 int rge_scratch_floats(void* hv) { return ((RgeHandle*)hv)->L.total; }
 int rge_small_bytes(void* hv) { return (int)((RgeHandle*)hv)->hm.small_bytes; }
-/* writable pointer to a model array (float32/int32 copy) so tests can edit parameters */
+/* writable pointer to a model array, the blob's or a derived one (float32/int32 copy), so tests can edit parameters */
 void* rge_model_field(void* hv, const char* name, int* count) {
-  RgeHandle* h = (RgeHandle*)hv;
-  RgModel& m = h->hm.view;
-#define RG_DIM(n) const int n = m.n; (void)n;
-#define RG_I(n, c)
-#define RG_F(n, c)
-#include "../../include/rg_model_fields.h"
-#undef RG_DIM
-#undef RG_I
-#undef RG_F
-#define RG_DIM(n)
-#define RG_I(n, c) if (!strcmp(name, #n)) { *count = (c); return (void*)m.n; }
-#define RG_F(n, c) if (!strcmp(name, #n)) { *count = (c); return (void*)m.n; }
-#include "../../include/rg_model_fields.h"
-#undef RG_DIM
-#undef RG_I
-#undef RG_F
-  return nullptr;
+  RgHostField f;
+  if (!rg_host_field(((RgeHandle*)hv)->hm.view, name, f)) return nullptr;
+  *count = (int)f.count;
+  return f.p;
 }
 
 void rge_step(void* hv, int nenv, float* qpos, float* qvel, float* ctrl, float* pid, float* warm, float* time, const float* xfrc,
@@ -108,13 +95,6 @@ void rge_step(void* hv, int nenv, float* qpos, float* qvel, float* ctrl, float* 
   if (h->sep.size() != (size_t)nenv * RG_NSEP) h->sep.assign((size_t)nenv * RG_NSEP, 0xfff);   /* like the engine's per-batch buffer */
   io.sep = h->sep.data();
   for (int env = 0; env < nenv; env++) rg_env_step(&h->hm.view, h->L, h->scratch.data(), 0, io, env, nsub, final_forward, 1);
-}
-
-/* ---- mesh scale: the engine-derived [nmesh] `mesh_scale` array (rg_host.h), which rge_model_field does not serve */
-float* rge_mesh_scale(void* hv, int* count) {
-  RgeHandle* h = (RgeHandle*)hv;
-  *count = h->hm.view.nmesh;
-  return (float*)h->hm.view.mesh_scale;
 }
 
 /* ---- per-environment pair lists (rg_batch_update_pairs)

@@ -58,7 +58,7 @@ def _scale_oracle(om, m, s):
 
 
 def _scale_emu(e, m, s):
-    e.mesh_scale()[:] = s
+    e.model_field("mesh_scale", np.float32)[:] = s
     e.model_field("geom_rbound", np.float32)[_mesh_geoms(m)] *= np.float32(s)
 
 
@@ -111,7 +111,7 @@ def test_explicit_unit_mesh_scale_is_bit_identical():
     for explicit in (False, True):
         e = pyemu.EmuBatch(blob, dims, 1)
         if explicit:
-            e.mesh_scale()[:] = 1.0
+            e.model_field("mesh_scale", np.float32)[:] = 1.0
         e.qpos[0], e.qvel[0], e.warm[0] = d.qpos, d.qvel, d.qacc_warmstart
         for _ in range(10):
             e.step(5, 1)
@@ -267,7 +267,7 @@ def test_emulated_full_cube_at_scale_1_05(full_states):
     e = pyemu.EmuBatch(blob, {k: m[k] for k in modelblob.DIMS}, n, **CAPS)
     e.model_field("body_pos", np.float32)[:] = _host_shifted_body_pos(blob, edited["body_pos"])
     e.model_field("geom_rbound", np.float32)[:] = edited["geom_rbound"]
-    e.mesh_scale()[mid] = 1.05
+    e.model_field("mesh_scale", np.float32)[mid] = 1.05
     for k in CONSTS:
         if np.asarray(edited[k]).size:
             e.model_field(k, np.float32)[:] = np.asarray(edited[k]).reshape(-1)
