@@ -24,8 +24,15 @@
 #include "rg_obs.inl"
 #include "rg_host.h"
 
+/* The step kernel is built twice.  Registers are granted to a CTA in groups of four warps, so 12 warps (384 threads) may
+   use 168 registers per thread, but 13 warps are granted the register file of 16 and get 128.  Up to RG_NARROW_WARPS warps
+   per CTA run the 168-register build; a batch takes RG_MAX_WARPS only where the extra warp saves a round (rg_batch_size).
+   Shared memory decides how many fit. */
 #ifndef RG_MAX_WARPS
-#define RG_MAX_WARPS 12   /* 168 registers x 384 threads fit the register file; shared memory decides how many are used */
+#define RG_MAX_WARPS 13
+#endif
+#ifndef RG_NARROW_WARPS
+#define RG_NARROW_WARPS 12
 #endif
 
 static thread_local std::string g_err;
@@ -63,7 +70,8 @@ __device__ __forceinline__ uint32_t rg_smem_u32(const void* p) { return (uint32_
 /* every warp with overrides keeps its own copy of the view: 128 B more would cost dactyl/locked a resident environment per SM */
 static_assert(sizeof(RgModelDev) <= 1024, "the device model view must fit in 1024 bytes of shared memory");
 
-__global__ void __launch_bounds__(RG_MAX_WARPS * 32, 1) rg_step_kernel(const __grid_constant__ RgKernelArgs args) {
+template <int MAXW>
+__global__ void __launch_bounds__(MAXW * 32, 1) rg_step_kernel(const __grid_constant__ RgKernelArgs args) {
   unsigned char* smem_raw = rg_smem_raw;
   __shared__ __align__(8) unsigned long long mbar;
   /* dynamic shared layout: [RgModelDev] [small model arena] [warps x scratch] [warps x (RgModelDev + override rows)] */
@@ -557,7 +565,7 @@ static int rg_batch_size(rg_batch* b) {
   RG_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device));
   RG_CUDA(cudaDeviceGetAttribute(&maxsmem, cudaDevAttrMaxSharedMemoryPerBlockOptin, m->device));
   cudaFuncAttributes fa;
-  RG_CUDA(cudaFuncGetAttributes(&fa, rg_step_kernel));
+  RG_CUDA(cudaFuncGetAttributes(&fa, rg_step_kernel<RG_MAX_WARPS>));   /* both builds declare the same static shared memory */
   maxsmem -= (int)fa.sharedSizeBytes;   /* the opt-in limit covers static + dynamic shared memory */
   const int model_bytes = RG_MODEL_DEV_BYTES;
   const int fixed = model_bytes + (int)((m->hm.small_bytes + 127) & ~(size_t)127) + 64;
@@ -568,6 +576,10 @@ static int rg_batch_size(rg_batch* b) {
   if (warps > RG_MAX_WARPS) warps = RG_MAX_WARPS;
   /* rounds are handed out dynamically and a partial round runs with fewer warps, so more resident warps never cost padding */
   if (warps > nenv) warps = nenv;
+  /* past RG_NARROW_WARPS every warp has fewer registers (see RG_MAX_WARPS): worth it only where the launch takes fewer rounds.
+     dactyl/locked's 8192 environments take 5 rounds of 132 x 13 instead of 6 of 132 x 12 */
+  if (warps > RG_NARROW_WARPS && (nenv + sms * warps - 1) / (sms * warps) >= (nenv + sms * RG_NARROW_WARPS - 1) / (sms * RG_NARROW_WARPS))
+    warps = RG_NARROW_WARPS;
   /* a batch smaller than one full round is spread over all SMs (fewer warps per CTA) rather than packed into few of them:
      a round lasts as long as its slowest environment, and fewer resident warps make every one of them faster */
   if (nenv < sms * warps) { const int even = (nenv + sms - 1) / sms; if (even < warps) warps = even; }
@@ -583,7 +595,8 @@ static int rg_batch_size(rg_batch* b) {
   b->ctas = ctas;
   /* the attribute belongs to the kernel, not to this batch: batches with different footprints coexist, so opt in to the
      device maximum once rather than to this batch's size */
-  RG_CUDA(cudaFuncSetAttribute(rg_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsmem));
+  RG_CUDA(cudaFuncSetAttribute(rg_step_kernel<RG_NARROW_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsmem));
+  RG_CUDA(cudaFuncSetAttribute(rg_step_kernel<RG_MAX_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsmem));
   return 0;
 }
 
@@ -844,7 +857,8 @@ static int rg_launch_step(rg_batch* b, const uint8_t* mask, int nsub, int final_
   }
   args.counter = b->d_counter;
   RG_CUDA(cudaMemsetAsync(b->d_counter, 0, sizeof(int), (cudaStream_t)stream));
-  rg_step_kernel<<<b->ctas, RG_MAX_WARPS * 32 < b->warps * 32 ? RG_MAX_WARPS * 32 : b->warps * 32, b->smem, (cudaStream_t)stream>>>(args);
+  if (b->warps > RG_NARROW_WARPS) rg_step_kernel<RG_MAX_WARPS><<<b->ctas, 32 * b->warps, b->smem, (cudaStream_t)stream>>>(args);
+  else rg_step_kernel<RG_NARROW_WARPS><<<b->ctas, 32 * b->warps, b->smem, (cudaStream_t)stream>>>(args);
   RG_CUDA(cudaGetLastError());
   if (!mask && b->balance && nsub > 0) {   /* (not after rg_set_const: it leaves no cost) */
     rg_order_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(b->d_cost, b->d_order, b->nenv);
