@@ -131,6 +131,11 @@ __device__ __forceinline__ void rg_stage_sync() {
 #define RG_GRP 8           /* lanes that share one pair in the convex-convex narrow phase (rg_mpr_batch) */
 #endif
 #define RG_NSEP 64         /* words of the per-environment separating-axis cache (rg_mpr_batch) */
+/* word offsets in the collision stage's narrow-phase staging area (L.stage, sized by rg_make_layout): [32][8] results of the
+   convex-convex pairs from 0, their 32 candidate slots from RG_STAGE_SLOTS, the two geom views of each lane group's pair
+   (rg_mpr_batch) from RG_STAGE_VIEWS */
+#define RG_STAGE_SLOTS 256
+#define RG_STAGE_VIEWS 288
 #ifndef RG_CELLN
 #define RG_CELLN 8         /* cells per cube-face edge of the hull support lists (rg_host_hull_cells, rg_hull_cell) */
 #endif

@@ -26,7 +26,8 @@
 
 /* The step kernel is built twice.  Registers are granted to a CTA in groups of four warps, so 12 warps (384 threads) may
    use 168 registers per thread, but 13 warps are granted the register file of 16 and get 128.  Up to RG_NARROW_WARPS warps
-   per CTA run the 168-register build; a batch takes RG_MAX_WARPS only where the extra warp saves a round (rg_batch_size).
+   per CTA run the 168-register build; a batch takes RG_MAX_WARPS only where the extra warp saves a round (rg_batch_size):
+   held at 12 warps, the 128-register build is still about 5 % slower per warp (DESIGN.md section 4, "Residency").
    Shared memory decides how many fit. */
 #ifndef RG_MAX_WARPS
 #define RG_MAX_WARPS 13
