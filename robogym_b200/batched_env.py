@@ -56,12 +56,14 @@ class ShadowHandCubeFacade:
         sn = names["site"]
         self.tip_sites = t([sn.index(hand_prefix + s) for s in FINGERTIP_SITES], torch.long)
         self.ref_sites = t([sn.index(hand_prefix + s) for s in REFERENCE_SITES], torch.long)
-        self.cube_center = sn.index(cube_prefix + "center")
+        # a model without a cube (dactyl/reach) has no cube observations and no on-palm test
+        self.has_cube = cube_prefix + "center" in sn
+        self.cube_center = sn.index(cube_prefix + "center") if self.has_cube else None
         cube_t = [j for j, n in enumerate(jn) if n is not None and n.startswith(cube_prefix + "cube_t")]
         cube_r = [j for j, n in enumerate(jn) if n == cube_prefix + "cube_rot"]
         self.cube_pos_idx = t([m["jnt_qposadr"][j] for j in cube_t], torch.long)
-        a = int(m["jnt_qposadr"][cube_r[0]])
-        self.cube_quat_idx = t(list(range(a, a + 4)), torch.long)
+        a = int(m["jnt_qposadr"][cube_r[0]]) if cube_r else 0
+        self.cube_quat_idx = t(list(range(a, a + 4)) if cube_r else [], torch.long)
         self.occlusion_geoms = t([g for g, n in enumerate(names["geom"]) if n is not None and n.endswith("occlusion")], torch.long)
 
     # ---- a6: action -> ctrl
@@ -96,18 +98,23 @@ class ShadowHandCubeFacade:
         basis = torch.stack([e0, ort, e2], dim=2)          # columns, like np.transpose([e0, ort, e2])
         return torch.bmm(tips, basis)
 
+    def fingertip_absolute_positions(self, site_xpos):
+        """MujocoShadowhandAbsoluteFingertipsObservation (envs/dactyl/observation/shadow_hand.py:40-58): [nenv, 15]"""
+        return site_xpos[:, self.tip_sites].reshape(site_xpos.shape[0], -1)
+
     def observe(self, qpos, qvel, site_xpos, act_force=None):
         torch = self.torch
-        quat = qpos[:, self.cube_quat_idx]
         obs = dict(
-            cube_pos=qpos[:, self.cube_pos_idx],          # get_qpos("cube_position"): slide-joint coordinates
-            # robogym.utils.rotation.quat_normalize (rotation.py:281-286) only canonicalises the sign (w >= 0)
-            cube_quat=quat * torch.where(quat[:, :1] < 0, -torch.ones_like(quat[:, :1]), torch.ones_like(quat[:, :1])),
             hand_angle=qpos[:, self.hand_qpos_idx],
             hand_velocity=qvel[:, self.hand_qvel_idx],
             fingertip_pos=self.fingertip_relative_positions(site_xpos).reshape(qpos.shape[0], -1),
             qpos=qpos, qvel=qvel,
         )
+        if self.has_cube:
+            quat = qpos[:, self.cube_quat_idx]
+            obs["cube_pos"] = qpos[:, self.cube_pos_idx]          # get_qpos("cube_position"): slide-joint coordinates
+            # robogym.utils.rotation.quat_normalize (rotation.py:281-286) only canonicalises the sign (w >= 0)
+            obs["cube_quat"] = quat * torch.where(quat[:, :1] < 0, -torch.ones_like(quat[:, :1]), torch.ones_like(quat[:, :1]))
         if act_force is not None:
             # normalize_by_limits (robot/shadow_hand/hand_utils.py:21-28): x / hi for x >= 0, |x| / lo otherwise
             obs["actuator_force"] = torch.where(act_force >= 0, act_force / self.force_hi, act_force.abs() / self.force_lo)

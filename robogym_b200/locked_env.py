@@ -105,6 +105,54 @@ class TorchRand:
         return self.torch.randint(0, hi, (n,), device=self.device, generator=self.gen)
 
 
+def track_goals(env, success, dtype):
+    """MultiGoalTracker.process (robogym/utils/multi_goal_tracker.py:157-241) for every environment of `env` (a batched dactyl
+    environment: its tracker tensors are updated in place).  success_pause_range_s is (0, 0) when the tracker is built, so one
+    successful step counts.  Returns (sub_goal_is_successful, success reward, done, trial_success, new-goal mask)."""
+    torch = env.torch
+    env.steps_since_last_goal += 1
+    env.consecutive_success = torch.where(success, env.consecutive_success + 1, torch.zeros_like(env.consecutive_success))
+    got = (env.consecutive_success >= 1) & ~env.success_pending
+    success_reward = got.to(dtype) * env.success_reward
+    env.successes_so_far += got.long()
+    env.success_pending |= got
+    done = ~got & (env.steps_since_last_goal >= env.max_timesteps_per_goal)
+    settle = env.success_pending & (env.steps_since_last_goal >= env.min_timesteps_per_goal)
+    env.success_pending &= ~settle
+    trial_success = settle & (env.successes_so_far >= env.successes_needed)
+    done |= trial_success
+    env.steps_since_last_goal[trial_success] = 0
+    return got, success_reward, done, trial_success, settle & ~trial_success
+
+
+class ActionLatency:
+    """RandomizedActionLatency (robogym/wrappers/randomizations.py:516-556): every action COORDINATE is delayed by 0..max_delay
+    env-steps, drawn per episode."""
+
+    def __init__(self, torch, rand, nenv, nu, max_delay, dtype, device):
+        self.torch, self.rand, self.max_delay = torch, rand, int(max_delay)
+        self.history = torch.zeros(nenv, self.max_delay + 1, nu, dtype=dtype, device=device)
+        self.delay = torch.zeros(nenv, nu, dtype=torch.long, device=device)
+
+    def reset(self, idx):
+        k = int(idx.numel())
+        self.history[idx] = 0
+        self.delay[idx] = self.rand.randint(self.max_delay + 1, k * self.delay.shape[1]).reshape(k, -1)
+
+    def __call__(self, a):
+        # The reference shifts its history with a tuple assignment whose right-hand side is a VIEW (randomizations.py:546-549):
+        # history[0] = action is visible to the shift that follows, so the result is [a, a, old[1], old[2], ...] -- a delay of
+        # d >= 1 returns the action of d - 1 steps ago (and the default max_delay = 1 delays nothing).  Reproduced as is: this
+        # is a drop-in, not a correction.
+        torch = self.torch
+        self.history.copy_(torch.cat([a.unsqueeze(1), a.unsqueeze(1), self.history[:, 1:-1]], dim=1))
+        return torch.gather(self.history, 1, self.delay.unsqueeze(1)).squeeze(1)
+
+    def observe(self, obs):
+        obs["action_history"] = self.history[:, :-1].clone()
+        obs["action_delay"] = self.delay.clone()
+
+
 STATE_FIELDS = ("qpos", "qvel", "ctrl", "pid", "qacc_warmstart", "time", "site_xpos", "act_force")
 
 
@@ -267,14 +315,11 @@ class BatchedLockedEnv:
         self.success_pending = z(torch.bool)        # MultiGoalTracker._success_and_no_goal_reset
         self.first_drop = z(torch.long)             # StopOnFallWrapper.first_drop
         self.episodes = 0
-        # RandomizedActionLatency (robogym/wrappers/randomizations.py:516-556; first entry of locked.py:265-277's stack, so it is
-        # on whenever the stack is): every action COORDINATE is delayed by 0..max_delay env-steps, drawn per episode
+        # RandomizedActionLatency: first entry of locked.py:265-277's stack, so it is on whenever the stack is
         if action_latency is None:
             action_latency = 1 if randomize else 0
-        self.max_delay = int(action_latency)
-        nu = int(model["nu"])
-        self.action_history = torch.zeros(n, self.max_delay + 1, nu, dtype=dtype, device=device)
-        self.action_delay = torch.zeros(n, nu, dtype=torch.long, device=device)
+        self.latency = ActionLatency(torch, self.rand, n, int(model["nu"]), action_latency, dtype, device)
+        self.max_delay, self.action_history, self.action_delay = self.latency.max_delay, self.latency.history, self.latency.delay
 
     # ---------------------------------------------------------------- goals
     def sample_goals(self, n):
@@ -326,8 +371,7 @@ class BatchedLockedEnv:
         if self.obs_noise is not None:              # RandomizeObservationWrapper.reset: new per-episode biases
             self.obs_noise.reset(idx)
         if self.max_delay > 0:                      # RandomizedActionLatency.reset
-            self.action_history[idx] = 0
-            self.action_delay[idx] = self.rand.randint(self.max_delay + 1, k * self.action_delay.shape[1]).reshape(k, -1)
+            self.latency.reset(idx)
         self.t[idx] = 0
         self.successes_so_far[idx] = 0
         self.goals_so_far[idx] = 0
@@ -359,8 +403,7 @@ class BatchedLockedEnv:
         obs["qpos_goal"] = qg
         obs["is_goal_achieved"] = (self.goal_distance() < self.success_threshold).to(s.qpos.dtype)
         if self.max_delay > 0:
-            obs["action_history"] = self.action_history[:, :-1].clone()
-            obs["action_delay"] = self.action_delay.clone()
+            self.latency.observe(obs)
         if self.obs_noise is not None:
             obs = self.obs_noise(obs)
         return obs
@@ -375,12 +418,7 @@ class BatchedLockedEnv:
         s = self.sim
         a = torch.clamp(torch.as_tensor(action, dtype=s.qpos.dtype, device=self.device), -1.0, 1.0)
         if self.max_delay > 0:
-            # RandomizedActionLatency.step.  The reference shifts its history with a tuple assignment whose right-hand side is
-            # a VIEW (randomizations.py:546-549): history[0] = action is visible to the shift that follows, so the result is
-            # [a, a, old[1], old[2], ...] -- a delay of d >= 1 returns the action of d - 1 steps ago (and the default
-            # max_delay = 1 delays nothing).  Reproduced as is: this is a drop-in, not a correction.
-            self.action_history = torch.cat([a.unsqueeze(1), a.unsqueeze(1), self.action_history[:, 1:-1]], dim=1)
-            a = torch.gather(self.action_history, 1, self.action_delay.unsqueeze(1)).squeeze(1)
+            a = self.latency(a)                     # RandomizedActionLatency.step
         cr = None
         if self.randomizer is not None:
             cr = s._params["actuator_ctrlrange"].reshape(self.nenv, -1, 2)
@@ -396,20 +434,7 @@ class BatchedLockedEnv:
         goal_reward = prev - dist
         self.prev_dist = dist.clone()
         success = dist < self.success_threshold
-        # MultiGoalTracker.process
-        self.steps_since_last_goal += 1
-        self.consecutive_success = torch.where(success, self.consecutive_success + 1, torch.zeros_like(self.consecutive_success))
-        got = (self.consecutive_success >= 1) & ~self.success_pending      # success_pause_range_s = (0, 0): one step suffices
-        success_reward = got.to(dist.dtype) * self.success_reward
-        self.successes_so_far += got.long()
-        self.success_pending |= got
-        done = ~got & (self.steps_since_last_goal >= self.max_timesteps_per_goal)
-        settle = self.success_pending & (self.steps_since_last_goal >= self.min_timesteps_per_goal)
-        self.success_pending &= ~settle
-        trial_success = settle & (self.successes_so_far >= self.successes_needed)
-        done |= trial_success
-        self.steps_since_last_goal[trial_success] = 0
-        newgoal = settle & ~trial_success
+        got, success_reward, done, trial_success, newgoal = track_goals(self, success, dist.dtype)
         info = dict(goal_dist=dist, goal_achieved=success, sub_goal_is_successful=got, trial_success=trial_success,
                     goal_reset=newgoal.clone(), successes_so_far=self.successes_so_far.clone())
         self._set_new_goal(newgoal, None if new_goals is None else torch.as_tensor(new_goals, dtype=dist.dtype, device=self.device)[newgoal])

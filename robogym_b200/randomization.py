@@ -132,14 +132,26 @@ def tendon_range_rule(torch, orig, noise, relative_std=0.15):
     return torch.stack([lo, hi], dim=-1)
 
 
+# The per-episode rules sample() draws.  The per-step rules (RandomizedTimestepWrapper, cube.RandomizedWindWrapper) are run by the
+# environments through timestep_state / next_timestep and wind_state / next_wind, and are not listed.  "set_constants" is
+# CubeEnv._reset's set_constants() (cube_env.py:343-349): the constants mj_setConst derives from the drawn inertias.
+LOCKED_RULES = ("body_inertia", "robot_friction", "cube_friction", "gravity", "joint_limit", "tendon_range", "phasespace",
+                "robot_damping", "robot_kp", "cube_size", "set_constants")
+# dactyl/reach's stack (reach.py:226-240): RandomizedActionLatency and the observation noise live in the environment.  Its reset
+# never calls set_constants() (RobotEnv._reset is `pass`), so the derived constants keep the model's values.
+REACH_RULES = ("body_inertia", "robot_friction", "gravity", "phasespace", "robot_damping", "robot_kp")
+CUBE_RULES = ("cube_friction", "cube_size")
+
+
 class LockedRandomizer:
-    """The randomisation stack of dactyl/locked (locked.py:263-277), drawn for n environments at once."""
+    """The randomisation stack of dactyl/locked (locked.py:263-277), drawn for n environments at once.  `rules` names the
+    wrappers of another dactyl stack (REACH_RULES); the cube's rules are skipped on a model without a cube."""
 
     EPISODE_PARAMS = ("body_inertia", "geom_friction", "opt_gravity", "dof_damping", "actuator_gainprm", "jnt_range",
                       "actuator_ctrlrange", "tendon_range", "geom_size", "geom_rbound", "geom_aabb", "site_pos",
                       "dof_invweight0", "body_invweight0", "tendon_invweight0", "opt_meaninertia")
 
-    def __init__(self, m, names, rand, torch, device, dtype, hand_prefix="robot0:", cube_prefix="cube:"):
+    def __init__(self, m, names, rand, torch, device, dtype, hand_prefix="robot0:", cube_prefix="cube:", rules=LOCKED_RULES):
         self.torch, self.rand, self.m = torch, rand, m
         self.device, self.dtype = device, dtype
         t = lambda a, dt=dtype: torch.as_tensor(np.asarray(a), dtype=dt, device=device)
@@ -176,8 +188,11 @@ class LockedRandomizer:
         self.constants = BatchedConstants(m, torch, device, dtype)
         self.timestep0 = float(m["opt_timestep"][0])
         self.nsub_dt = None
-        self.cube_body = names["body"].index(cube_prefix + "middle")
-        self.cube_mass = float(m["body_mass"][self.cube_body])
+        has_cube = cube_prefix + "middle" in names["body"]
+        self.rules = tuple(r for r in rules if has_cube or r not in CUBE_RULES)
+        if has_cube:
+            self.cube_body = names["body"].index(cube_prefix + "middle")
+            self.cube_mass = float(m["body_mass"][self.cube_body])
 
     def _logu(self, lo, hi, n, k):
         return self.torch.exp(self.rand.uniform(math.log(lo), math.log(hi), n, k))
@@ -189,38 +204,48 @@ class LockedRandomizer:
         nz = noises or {}
         draw = lambda key, fn: nz[key].to(self.dtype) if key in nz else fn()
         out = {}
+        on = self.rules
         nb = m["nbody"]
-        out["body_inertia"] = (o["body_inertia"].reshape(1, nb, 3) * draw("inertia", lambda: self.rand.uniform(0.5, 1.5, n, nb)).unsqueeze(2)).reshape(n, -1)
-        fr = o["geom_friction"].reshape(1, -1, 3).repeat(n, 1, 1)
-        rm = draw("robot_friction", lambda: torch.stack([self.rand.uniform(a, b, n, 1)[:, 0] for a, b in ((0.7, 1.3), (0.5, 1.5), (0.5, 1.5))], dim=1))
-        cm = draw("cube_friction", lambda: torch.stack([self.rand.uniform(a, b, n, 1)[:, 0] for a, b in ((0.5, 1.5), (0.2, 5.0), (0.2, 5.0))], dim=1))
-        fr[:, self.robot_geoms] = fr[:, self.robot_geoms] * rm.unsqueeze(1)
-        fr[:, self.cube_geoms] = fr[:, self.cube_geoms] * cm.unsqueeze(1)
-        out["geom_friction"] = fr.reshape(n, -1)
-        out["opt_gravity"] = o["opt_gravity"] + 0.4 * draw("gravity", lambda: self.rand.randn(n, 3))
-        damp = o["dof_damping"].repeat(n, 1)
-        damp[:, self.robot_dofs] = damp[:, self.robot_dofs] * draw("damping", lambda: self._logu(1 / 1.5, 1.5, n, int(self.robot_dofs.numel())))
-        out["dof_damping"] = damp
-        gain = o["actuator_gainprm"].reshape(1, m["nu"], -1).repeat(n, 1, 1)
-        gain[:, self.robot_acts, 0] = gain[:, self.robot_acts, 0] * draw("kp", lambda: self._logu(0.5, 2.0, n, int(self.robot_acts.numel())))
-        out["actuator_gainprm"] = gain.reshape(n, -1)
-        # joint limits (robot joints) and the control ranges that follow them
-        nj = m["njnt"]
-        jr = joint_limit_rule(torch, self.joint_limits0.repeat(n, 1, 1), draw("joint_limit", lambda: self.rand.randn(n, nj * 2).reshape(n, nj, 2)))
-        out["jnt_range"] = jr.reshape(n, -1)
-        cr = o["actuator_ctrlrange"].reshape(1, -1, 2).repeat(n, 1, 1)
-        for j, a, other in self.act_of_joint:
-            if other >= 0:
-                cr[:, a, 0] = torch.minimum(jr[:, other, 0], jr[:, j, 0])
-                cr[:, a, 1] = jr[:, other, 1] + jr[:, j, 1]
-            else:
-                cr[:, a] = jr[:, j]
-        out["actuator_ctrlrange"] = cr.reshape(n, -1)
-        nt = m["ntendon"]
-        out["tendon_range"] = tendon_range_rule(torch, o["tendon_range"].reshape(1, nt, 2).repeat(n, 1, 1),
-                                                draw("tendon_range", lambda: self.rand.randn(n, nt * 2).reshape(n, nt, 2))).reshape(n, -1)
+        if "body_inertia" in on:
+            out["body_inertia"] = (o["body_inertia"].reshape(1, nb, 3) * draw("inertia", lambda: self.rand.uniform(0.5, 1.5, n, nb)).unsqueeze(2)).reshape(n, -1)
+        if "robot_friction" in on or "cube_friction" in on:
+            fr = o["geom_friction"].reshape(1, -1, 3).repeat(n, 1, 1)
+            if "robot_friction" in on:
+                rm = draw("robot_friction", lambda: torch.stack([self.rand.uniform(a, b, n, 1)[:, 0] for a, b in ((0.7, 1.3), (0.5, 1.5), (0.5, 1.5))], dim=1))
+                fr[:, self.robot_geoms] = fr[:, self.robot_geoms] * rm.unsqueeze(1)
+            if "cube_friction" in on:
+                cm = draw("cube_friction", lambda: torch.stack([self.rand.uniform(a, b, n, 1)[:, 0] for a, b in ((0.5, 1.5), (0.2, 5.0), (0.2, 5.0))], dim=1))
+                fr[:, self.cube_geoms] = fr[:, self.cube_geoms] * cm.unsqueeze(1)
+            out["geom_friction"] = fr.reshape(n, -1)
+        if "gravity" in on:
+            out["opt_gravity"] = o["opt_gravity"] + 0.4 * draw("gravity", lambda: self.rand.randn(n, 3))
+        if "robot_damping" in on:
+            damp = o["dof_damping"].repeat(n, 1)
+            damp[:, self.robot_dofs] = damp[:, self.robot_dofs] * draw("damping", lambda: self._logu(1 / 1.5, 1.5, n, int(self.robot_dofs.numel())))
+            out["dof_damping"] = damp
+        if "robot_kp" in on:
+            gain = o["actuator_gainprm"].reshape(1, m["nu"], -1).repeat(n, 1, 1)
+            gain[:, self.robot_acts, 0] = gain[:, self.robot_acts, 0] * draw("kp", lambda: self._logu(0.5, 2.0, n, int(self.robot_acts.numel())))
+            out["actuator_gainprm"] = gain.reshape(n, -1)
+        if "joint_limit" in on:
+            # joint limits (robot joints) and the control ranges that follow them
+            nj = m["njnt"]
+            jr = joint_limit_rule(torch, self.joint_limits0.repeat(n, 1, 1), draw("joint_limit", lambda: self.rand.randn(n, nj * 2).reshape(n, nj, 2)))
+            out["jnt_range"] = jr.reshape(n, -1)
+            cr = o["actuator_ctrlrange"].reshape(1, -1, 2).repeat(n, 1, 1)
+            for j, a, other in self.act_of_joint:
+                if other >= 0:
+                    cr[:, a, 0] = torch.minimum(jr[:, other, 0], jr[:, j, 0])
+                    cr[:, a, 1] = jr[:, other, 1] + jr[:, j, 1]
+                else:
+                    cr[:, a] = jr[:, j]
+            out["actuator_ctrlrange"] = cr.reshape(n, -1)
+        if "tendon_range" in on:
+            nt = m["ntendon"]
+            out["tendon_range"] = tendon_range_rule(torch, o["tendon_range"].reshape(1, nt, 2).repeat(n, 1, 1),
+                                                    draw("tendon_range", lambda: self.rand.randn(n, nt * 2).reshape(n, nt, 2))).reshape(n, -1)
         # cube size: geom_size of cube:middle and the bounds the broad phase derives from it
-        if self.cube_middle is not None:
+        if "cube_size" in on and self.cube_middle is not None:
             scale = draw("cube_size", lambda: self.rand.uniform(0.95, 1.05, n, 1))
             gs = o["geom_size"].reshape(1, -1, 3).repeat(n, 1, 1)
             gs[:, self.cube_middle] = gs[:, self.cube_middle] * scale
@@ -232,12 +257,14 @@ class LockedRandomizer:
             ab[:, self.cube_middle, 3:6] = gs[:, self.cube_middle]
             out["geom_aabb"] = ab.reshape(n, -1)
         self._extra_rules(n, draw, out)
-        # phasespace marker sites
-        sp = o["site_pos"].reshape(1, -1, 3).repeat(n, 1, 1)
-        sp[:, self.tip_sites] += 0.003 * draw("tip_noise", lambda: self.rand.randn(n, 15).reshape(n, 5, 3))
-        sp[:, self.ref_sites] += 0.001 * draw("ref_noise", lambda: self.rand.randn(n, 9).reshape(n, 3, 3))
-        out["site_pos"] = sp.reshape(n, -1)
-        out.update(self.constants.derive(out["body_inertia"]))
+        if "phasespace" in on:
+            # phasespace marker sites
+            sp = o["site_pos"].reshape(1, -1, 3).repeat(n, 1, 1)
+            sp[:, self.tip_sites] += 0.003 * draw("tip_noise", lambda: self.rand.randn(n, 15).reshape(n, 5, 3))
+            sp[:, self.ref_sites] += 0.001 * draw("ref_noise", lambda: self.rand.randn(n, 9).reshape(n, 3, 3))
+            out["site_pos"] = sp.reshape(n, -1)
+        if "set_constants" in on and "body_inertia" in out:
+            out.update(self.constants.derive(out["body_inertia"]))
         return out
 
     def _extra_rules(self, n, draw, out):

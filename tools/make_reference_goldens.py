@@ -228,6 +228,144 @@ def full_perpendicular():
     return rec
 
 
+# ---------------------------------------------------------------- dactyl/reach (tests/test_reach_env.py)
+REACH_OBS_KEYS = ("qpos", "qvel", "fingertip_pos", "goal_fingertip_pos", "is_goal_achieved")
+
+
+def _count_calls(mj, counts):
+    """count mj_step / mj_forward calls of one MjSim in `counts` (mujoco-py's PID state advances in each)"""
+    for name in ("step", "forward"):
+        real = getattr(mj, name)
+
+        def spy(*a, _real=real, _name=name, **kw):
+            counts[_name] += 1
+            return _real(*a, **kw)
+
+        setattr(mj, name, spy)
+
+
+def reach():
+    """ReachEnv (make_simple_env) with small tracker constants: both simulations after the build, every RandomState.normal draw of
+    FingertipPosGoal.next_goal with the goal it produced, an episode reset, forced successes, a trial success, a timeout, the
+    mj_step / mj_forward counts of both simulations per phase, FingerSeparationWrapper's jnt_range for every active_finger, and
+    which model arrays reach's randomisation stack changes on which simulation"""
+    from robogym.envs.dactyl.goals.shadow_hand_reach_fingertip_pos import FingertipPosGoal
+    from robogym.envs.dactyl.reach import make_env, make_simple_env
+    from robogym.wrappers import dactyl as dw
+
+    draws = []
+    real_next_goal = FingertipPosGoal.next_goal
+
+    class Normal:
+        def __init__(self, rs):
+            self.rs = rs
+
+        def normal(self, loc, scale):
+            v = self.rs.normal(loc=loc, scale=scale)
+            draws.append(dict(loc=_l(loc), scale=_l(scale), normal=_l(v)))
+            return v
+
+    def next_goal(self, random_state, current_state):
+        if not draws:
+            out["goal_build"] = _sim_state(self.goal_simulation.mj_sim)
+        goal = real_next_goal(self, Normal(random_state), current_state)
+        draws[-1].update(fingertip_pos=_l(goal["fingertip_pos"]), goal_joint_pos=_l(self.goal_joint_pos), goal_state=_sim_state(self.goal_simulation.mj_sim))
+        return goal
+
+    out = {}
+    FingertipPosGoal.next_goal = next_goal
+    try:
+        consts = dict(max_timesteps_per_goal=6, successes_needed=2)
+        env = make_simple_env(starting_seed=5, constants=consts)
+        ms, gs = env.mujoco_simulation, env.goal_generation.goal_simulation
+        main_n, goal_n = dict(step=0, forward=0), dict(step=0, forward=0)
+        _count_calls(ms.mj_sim, main_n)
+        _count_calls(gs.mj_sim, goal_n)
+        tr = env.multi_goal_tracker
+        out.update(constants=consts, main_build=_sim_state(ms.mj_sim), nsubsteps=int(ms.mj_sim.nsubsteps),
+                   goal_joint_pos0=draws[0]["loc"], goal_margin_added=_l(gs.mj_sim.model.geom_margin - ms.mj_sim.model.geom_margin),
+                   success_steps_required_built=int(tr._success_steps_required), success_threshold=float(env.constants.success_threshold["fingertip_pos"]),
+                   relative_action=bool(env.constants.relative_action), success_reward=float(env.constants.success_reward))
+
+        def counts():
+            c = dict(main=dict(main_n), goal=dict(goal_n))
+            for d in (main_n, goal_n):
+                d.update(step=0, forward=0)
+            return c
+
+        def tracker():
+            return dict(steps_since_last_goal=int(tr._steps_since_last_goal), consecutive_success=int(tr._consecutive_steps_with_success),
+                        successes_so_far=int(tr._successes_so_far), goals_so_far=int(tr._goals_so_far), success_pending=bool(tr._success_and_no_goal_reset),
+                        success_steps_required=int(tr._success_steps_required))
+
+        def record_reset():
+            n0 = len(draws)
+            counts()
+            obs = env.reset()
+            return dict(draws=list(range(n0, len(draws))), calls=counts(), main_state=_sim_state(ms.mj_sim), goal_state=_sim_state(gs.mj_sim),
+                        obs={k: _l(obs[k]) for k in REACH_OBS_KEYS}, goal=_l(env._goal["fingertip_pos"]), prev_dist=float(env._previous_goal_distance["fingertip_pos"]),
+                        tracker=tracker(), success_pause_range_s=list(env.constants.success_pause_range_s))
+
+        out["draws_at_construction"] = len(draws)
+        out["reset"] = record_reset()
+        steps = []
+        rng = np.random.RandomState(1)
+        episode_ends = 0
+        for k in range(40):
+            st = {}
+            if k in (1, 4):     # the goal put on the current fingertips: the next step succeeds
+                cur = env.goal_generation.current_state()["fingertip_pos"].copy()
+                env._goal["fingertip_pos"] = cur
+                st["goal_override"] = _l(cur)
+            a = rng.uniform(-1, 1, 20) * 0.3
+            n0 = len(draws)
+            obs, rew, done, info = env.step(a)
+            st.update(action=_l(a), draws=list(range(n0, len(draws))), calls=counts(), obs={key: _l(obs[key]) for key in REACH_OBS_KEYS},
+                      reward=_l(rew), done=bool(done), goal_dist=float(info["goal_dist"]["fingertip_pos"]), goal_reset=bool(info.get("goal_reset", False)),
+                      goal_achieved=bool(info["goal_achieved"]), main_state=_sim_state(ms.mj_sim),
+                      **{key: int(info[key]) for key in ("successes_so_far", "goals_so_far", "steps_since_last_goal")},
+                      **{key: bool(info[key]) for key in ("trial_success", "sub_goal_is_successful")})
+            steps.append(st)
+            if done:
+                episode_ends += 1
+                if episode_ends == 2:
+                    break
+                st["reset"] = record_reset()
+        out["steps"] = steps
+        out["draws"] = draws[:]
+    finally:
+        FingertipPosGoal.next_goal = real_next_goal
+
+    # FingerSeparationWrapper: jnt_range of the main simulation after the wrapper's reset, per active finger
+    env = make_simple_env(starting_seed=0)
+    jr0 = env.sim.model.jnt_range.copy()
+    out["jnt_range0"] = _l(jr0)
+    out["active_finger"] = {}
+    for finger in ("TH", "FF", "MF", "RF", "LF", "WR"):
+        env.sim.model.jnt_range[:] = jr0
+        dw.FingerSeparationWrapper(env, active_finger=finger).reset()
+        out["active_finger"][finger] = dict(main=_l(env.sim.model.jnt_range), goal=_l(env.goal_generation.goal_simulation.mj_sim.model.jnt_range))
+    env.sim.model.jnt_range[:] = jr0
+
+    # reach's randomisation stack (make_env(randomize=True)): which model arrays change on the main and on the goal simulation
+    from robogym_b200 import modelblob
+
+    env = make_env(starting_seed=0, constants=dict(randomize=True))
+    inner = env.unwrapped
+    mm, gm = inner.mujoco_simulation.mj_sim.model._cm, inner.goal_generation.goal_simulation.mj_sim.model._cm
+    before = (modelblob.unpack(mm.blob()), modelblob.unpack(gm.blob()))
+    env.reset()
+    after = (modelblob.unpack(mm.blob()), modelblob.unpack(gm.blob()))
+    out["randomized_fields"] = {side: sorted(k for _, k, _ in modelblob.ARRAYS if not np.array_equal(b[k], a[k]))
+                                for side, b, a in zip(("main", "goal"), before, after)}
+    w, chain = env, []
+    while hasattr(w, "env"):
+        chain.append(type(w).__name__)
+        w = w.env
+    out["wrappers"] = chain
+    return out
+
+
 # ---------------------------------------------------------------- observation noise (tests/test_obs_noise.py)
 class _Recorder:
     """numpy RandomState look-alike that logs what it hands out"""
@@ -369,7 +507,9 @@ def rearrange():
 def main():
     _engine()
     for name, fn in (("reference_locked", locked), ("reference_facade", facade), ("reference_full_perpendicular", full_perpendicular),
-                     ("reference_obs_noise", obs_noise), ("reference_rearrange", rearrange)):
+                     ("reference_obs_noise", obs_noise), ("reference_rearrange", rearrange), ("reference_reach", reach)):
+        if len(sys.argv) > 1 and name not in sys.argv[1:]:      # optional: regenerate only the named fixtures
+            continue
         rec = fn()
         path = os.path.join(GOLDEN, name + ".json.gz")
         with open(path, "wb") as f:      # mtime=0: the same record gives the same bytes
