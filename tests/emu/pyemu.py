@@ -31,6 +31,7 @@ def lib():
         L.rge_destroy.argtypes = [vp]
         for f in ("rge_dbg_size", "rge_scratch_floats", "rge_small_bytes", "rge_ncon", "rge_pidw"):
             getattr(L, f).argtypes = [vp]
+        L.rge_layout.argtypes = [vp, pi, ci]
         L.rge_name2id.argtypes = [vp, ctypes.c_char_p, ctypes.c_char_p]
         L.rge_model_field.restype = vp
         L.rge_model_field.argtypes = [vp, ctypes.c_char_p, pi]
@@ -75,6 +76,28 @@ def philox_check():
     L.rg_philox_mismatches.restype = ctypes.c_longlong
     L.rg_philox_mismatches.argtypes = [ctypes.c_int, ctypes.c_uint32, ctypes.c_uint32]
     return L
+
+
+# RgLayout's members in declaration order (robogym_b200/csrc/rg_defs.h): float offsets into a warp's scratch, then the capacities
+LAYOUT_FIELDS = ("qpos", "qvel", "ctrl", "pid", "warm", "lpos", "lquat", "xpos", "xquat", "gxpos", "sxpos", "S", "M", "H", "Sdot", "I10",
+                 "crb", "bias", "smooth", "qacc", "Ma", "search", "Mv", "qfc", "tmp", "tlen", "tvel", "tJn", "tJi", "tJv", "alen", "aforce",
+                 "con", "cu", "cw", "cF", "cprm", "el_i", "el_D", "el_jar", "el_jv", "el_f", "tileJ", "tileWJ", "tileDof", "cand", "cand2",
+                 "scal", "eldof", "env", "cdof", "sep", "stage", "mocap", "ncon", "nel", "tile", "total")
+
+
+def layout(blob, ncon=0, nel=0, tile=0):
+    """the scratch layout rg_make_layout gives the model at these capacities (0 = engine default): {member: int}"""
+    h = lib().rge_create_ex(bytes(blob), len(blob), ncon, nel, tile)
+    if not h:
+        raise RuntimeError("rge_create failed")
+    try:
+        out = (ctypes.c_int * len(LAYOUT_FIELDS))()
+        n = lib().rge_layout(h, out, len(out))
+    finally:
+        lib().rge_destroy(h)
+    if n != len(LAYOUT_FIELDS):
+        raise RuntimeError(f"RgLayout has {n} members, LAYOUT_FIELDS names {len(LAYOUT_FIELDS)}")
+    return dict(zip(LAYOUT_FIELDS, out))
 
 
 def _p(a):

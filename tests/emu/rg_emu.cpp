@@ -75,6 +75,13 @@ void rge_set_const(void* hv, float* dof_invweight0, float* body_invweight0, floa
 void rge_destroy(void* hv) { delete (RgeHandle*)hv; }
 int rge_dbg_size(void* hv) { return rg_dbg_size(((RgeHandle*)hv)->hm.view, ((RgeHandle*)hv)->L.ncon); }
 int rge_scratch_floats(void* hv) { return ((RgeHandle*)hv)->L.total; }
+/* the handle's scratch layout (rg_make_layout) as ints in RgLayout's declaration order; returns how many it has (copies at most n) */
+int rge_layout(void* hv, int* out, int n) {
+  const RgLayout& L = ((RgeHandle*)hv)->L;
+  const int k = (int)(sizeof(RgLayout) / sizeof(int));
+  memcpy(out, &L, sizeof(int) * (size_t)(n < k ? n : k));
+  return k;
+}
 int rge_small_bytes(void* hv) { return (int)((RgeHandle*)hv)->hm.small_bytes; }
 /* writable pointer to a model array, the blob's or a derived one (float32/int32 copy), so tests can edit parameters */
 void* rge_model_field(void* hv, const char* name, int* count) {

@@ -74,6 +74,26 @@ def contract_states(blob, seeds, per_seed, settle=20, nsub=10):
     return states, after, om
 
 
+def full_cube_states(blob, n=16):
+    """dactyl/full_perpendicular on the oracle: 5 settling env-steps at mid-range targets, then n env-steps of smoothed random
+    targets.  Returns (states, after) like rollout_states."""
+    om, d = oracle_pair(blob)
+    nu = om.dim("nu")
+    cr = om.field("actuator_ctrlrange").reshape(-1, 2)
+    rng = np.random.RandomState(3)
+    d.ctrl[:] = cr.mean(1)
+    for _ in range(5):
+        d.env_step(10)
+    states, after = [], []
+    for _ in range(n):
+        a = rng.uniform(-1, 1, nu)
+        d.ctrl[:] = np.clip(d.ctrl + 0.3 * a * (cr[:, 1] - cr[:, 0]) / 2, cr[:, 0], cr[:, 1])
+        states.append((d.qpos.copy(), d.qvel.copy(), d.ctrl.copy(), d.userdata[:3 * nu].copy(), d.qacc_warmstart.copy()))
+        d.env_step(10)
+        after.append((d.qpos.copy(), d.qvel.copy(), int(d.ncon[0])))
+    return states, after
+
+
 def live_indices(om, names):
     """qpos / qvel indices excluding the free-falling, collision-less target cube
     (robogym/envs/dactyl/locked.py:89-96; masked from observations, observation/mujoco.py:46,60)."""

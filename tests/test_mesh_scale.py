@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 import pyemu
-from helpers import oracle_pair
+from helpers import full_cube_states, oracle_pair
 from robogym_b200 import mjcf, modelblob
 
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
@@ -187,22 +187,7 @@ def _cube_edits(m, names, s):
 @pytest.fixture(scope="module")
 def full_states():
     """teacher-forcing states built like tests/test_full_cube.py's fixture"""
-    blob, names, m = _full()
-    om, d = oracle_pair(blob)
-    nu = m["nu"]
-    cr = m["actuator_ctrlrange"].reshape(-1, 2)
-    rng = np.random.RandomState(3)
-    d.ctrl[:] = cr.mean(1)
-    for _ in range(5):
-        d.env_step(10)
-    states, after = [], []
-    for _ in range(16):
-        a = rng.uniform(-1, 1, nu)
-        d.ctrl[:] = np.clip(d.ctrl + 0.3 * a * (cr[:, 1] - cr[:, 0]) / 2, cr[:, 0], cr[:, 1])
-        states.append((d.qpos.copy(), d.qvel.copy(), d.ctrl.copy(), d.userdata[:3 * nu].copy(), d.qacc_warmstart.copy()))
-        d.env_step(10)
-        after.append((d.qpos.copy(), d.qvel.copy(), int(d.ncon[0])))
-    return states, after
+    return full_cube_states(_full()[0])
 
 
 def check(qpos, ncon, warn, after):
