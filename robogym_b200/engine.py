@@ -24,6 +24,85 @@ LIB_PATH = os.environ.get("RG_LIB", os.path.join(_HERE, "librobogym_b200.so"))  
 MAX_CONTACTS = 32
 CON_STRIDE = 24
 
+_vp, _ci, _cd, _u32, _str, _P = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_uint32, ctypes.c_char_p, ctypes.POINTER
+
+
+class GoalIn(ctypes.Structure):
+    """rg_goal_in (include/robogym_b200.h)"""
+    _fields_ = [("nenv", _ci), ("nobj", _ci), ("pos", _vp), ("quat", _vp), ("pos_stride", ctypes.c_longlong), ("quat_stride", ctypes.c_longlong),
+                ("rows", _vp), ("goal_pos", _vp), ("goal_quat", _vp), ("group", _vp), ("pos_offset", _vp), ("rot_weight", _vp), ("table", _cd * 6),
+                ("rot_dist_type", _ci), ("success_keys", _ci), ("pos_threshold", _cd), ("rot_threshold", _cd), ("reward_per_object", _cd)]
+
+
+class GoalOut(ctypes.Structure):
+    """rg_goal_out (include/robogym_b200.h)"""
+    _fields_ = [("obj_rot", _vp), ("rel_pos", _vp), ("rel_rot", _vp), ("dist_pos", _vp), ("dist_rot", _vp), ("success", _vp), ("off_table", _vp),
+                ("num_success", _vp), ("reward", _vp), ("achieved", _vp), ("any_off", _vp), ("pick", _vp)]
+
+
+class ObsIn(ctypes.Structure):
+    """rg_obs_in (include/robogym_b200.h)"""
+    _fields_ = [("nenv", _ci), ("nobj", _ci), ("body_xpos", _vp), ("body_xquat", _vp), ("body_xvel", _vp), ("qpos", _vp), ("qvel", _vp),
+                ("ctrl", _vp), ("sensordata", _vp), ("contact", _vp), ("ncon", _vp), ("nbody", _ci), ("nq", _ci), ("nv", _ci), ("nu", _ci),
+                ("nsensordata", _ci), ("ncontact", _ci), ("ngeom", _ci), ("obj_body", _vp), ("obj_qpos", _vp), ("tcp_body", _ci),
+                ("narm", _ci), ("arm_qpos", _ci * 8), ("ngrip", _ci), ("grip_qpos", _ci * 4), ("grip_qvel", _ci * 4), ("grip_act", _ci),
+                ("force_adr", _ci), ("torque_adr", _ci), ("geom_object", _vp), ("geom_flags", _vp), ("table_plane", _ci), ("wrist_sphere", _ci),
+                ("pad", _ci * 2), ("goal_pos", _vp), ("goal_quat", _vp), ("rel_pos", _vp), ("rel_rot", _vp), ("achieved", _vp), ("off_table", _vp),
+                ("group", _vp), ("qpos_at_goal", _vp), ("bbox_size", _vp), ("colors", _vp), ("boundary", _vp), ("penalty", _cd * 4),
+                ("mask_obs", _ci), ("mask_margin", _cd)]
+
+
+class ObsOut(ctypes.Structure):
+    """rg_obs_out (include/robogym_b200.h): one output pointer per observation key"""
+    _fields_ = [(k, _vp) for k in (
+        "obj_pos obj_rel_pos obj_vel_pos obj_rot obj_vel_rot robot_joint_pos gripper_pos gripper_velp gripper_controls gripper_qpos "
+        "gripper_vel qpos qpos_goal goal_obj_pos goal_obj_rot rel_goal_obj_pos rel_goal_obj_rot is_goal_achieved obj_gripper_contact "
+        "obj_bbox_size obj_colors safety_stop tcp_force tcp_torque placement_mask goal_placement_mask masked_obj_pos masked_obj_rot "
+        "masked_obj_rel_pos masked_obj_vel_pos masked_obj_vel_rot masked_obj_gripper_contact masked_obj_bbox_size masked_obj_colors "
+        "masked_goal_obj_pos masked_goal_obj_rot masked_rel_goal_obj_pos masked_rel_goal_obj_rot gripper_table_contact wrist_cam_contacts "
+        "sim_reward sim_done").split()]
+
+
+# name -> (restype, argtypes) of every function include/robogym_b200.h declares, in its order (tests/test_abi.py checks the
+# table against the header)
+SIGNATURES = {
+    "rg_model_load": (_ci, [_vp, ctypes.c_size_t, _ci, _P(_vp)]),
+    "rg_model_destroy": (None, [_vp]),
+    "rg_model_dim": (_ci, [_vp, _str]),
+    "rg_model_name2id": (_ci, [_vp, _str, _str]),
+    "rg_model_id2name": (_str, [_vp, _str, _ci]),
+    "rg_model_set_field": (_ci, [_vp, _str, _vp, ctypes.c_size_t]),
+    "rg_model_set_field_async": (_ci, [_vp, _str, _vp, ctypes.c_size_t, _vp]),
+    "rg_dbg_size": (_ci, [_vp]),
+    "rg_scratch_bytes": (_ci, [_vp]),
+    "rg_batch_create": (_ci, [_vp, _ci, _P(_vp)]),
+    "rg_batch_create_ex": (_ci, [_vp, _ci, _ci, _ci, _ci, _P(_vp)]),
+    "rg_batch_capacity": (_ci, [_vp, _P(_ci), _P(_ci), _P(_ci)]),
+    "rg_batch_dbg_size": (_ci, [_vp]),
+    "rg_batch_scratch_bytes": (_ci, [_vp]),
+    "rg_batch_destroy": (None, [_vp]),
+    "rg_batch_bind": (_ci, [_vp, _ci, _vp]),
+    "rg_batch_bind_param": (_ci, [_vp, _str, _vp]),
+    "rg_batch_update_pairs": (_ci, [_vp, _vp, _vp]),
+    "rg_batch_mark_pairs_stale": (_ci, [_vp, _vp, _vp]),
+    "rg_batch_set_pair_capacity": (_ci, [_vp, _ci]),
+    "rg_batch_pair_info": (_ci, [_vp, _P(_ci), _P(_vp)]),
+    "rg_model_origin": (_ci, [_vp, _P(ctypes.c_float)]),
+    "rg_batch_set_balance": (_ci, [_vp, _ci]),
+    "rg_batch_launch_info": (_ci, [_vp, _P(_ci), _P(_ci), _P(_ci)]),
+    "rg_step": (_ci, [_vp, _ci, _ci, _vp]),
+    "rg_forward": (_ci, [_vp, _vp]),
+    "rg_step_subset": (_ci, [_vp, _vp, _ci, _ci, _vp]),
+    "rg_set_const": (_ci, [_vp, _vp, _vp]),
+    "rg_reset": (_ci, [_vp, _vp, _vp]),
+    "rg_batch_body_aabb": (_ci, [_vp, _vp, _ci, _vp, _vp, _vp, _vp]),
+    "rg_place_objects": (_ci, [_ci, _ci, _vp, _vp, _vp, _vp, _ci, _ci, _ci, _cd, _cd, _vp, _u32, _u32, _vp, _vp, _vp, _vp]),
+    "rg_rearrange_goal": (_ci, [_P(GoalIn), _vp, _vp, _P(GoalOut), _vp]),
+    "rg_goal_orientations": (_ci, [_ci, _ci, _vp, _vp, _ci, _u32, _u32, _vp, _vp, _vp]),
+    "rg_rearrange_obs": (_ci, [_P(ObsIn), _vp, _P(ObsOut), _vp]),
+    "rg_last_error": (_str, []),
+}
+
 _lib = None
 
 
@@ -32,7 +111,7 @@ class EngineError(RuntimeError):
 
 
 def lib():
-    """Load librobogym_b200.so (built in-tree by `python -m robogym_b200.build`)."""
+    """Load librobogym_b200.so (built in-tree by `python -m robogym_b200.build`) with the signatures of SIGNATURES."""
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
@@ -41,38 +120,9 @@ def lib():
                 "(nvcc, sm_90a). There is no CPU fallback."
             )
         L = ctypes.CDLL(LIB_PATH)
-        vp, ci = ctypes.c_void_p, ctypes.c_int
-        L.rg_last_error.restype = ctypes.c_char_p
-        L.rg_model_load.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ci, ctypes.POINTER(vp)]
-        L.rg_model_destroy.argtypes = [vp]
-        L.rg_model_dim.argtypes = [vp, ctypes.c_char_p]
-        L.rg_model_set_field.argtypes = [vp, ctypes.c_char_p, vp, ctypes.c_size_t]
-        L.rg_model_set_field_async.argtypes = [vp, ctypes.c_char_p, vp, ctypes.c_size_t, vp]
-        L.rg_model_name2id.argtypes = [vp, ctypes.c_char_p, ctypes.c_char_p]
-        L.rg_model_id2name.argtypes = [vp, ctypes.c_char_p, ci]
-        L.rg_model_id2name.restype = ctypes.c_char_p
-        L.rg_dbg_size.argtypes = [vp]
-        L.rg_scratch_bytes.argtypes = [vp]
-        L.rg_batch_create.argtypes = [vp, ci, ctypes.POINTER(vp)]
-        L.rg_batch_create_ex.argtypes = [vp, ci, ci, ci, ci, ctypes.POINTER(vp)]
-        L.rg_batch_capacity.argtypes = [vp, ctypes.POINTER(ci), ctypes.POINTER(ci), ctypes.POINTER(ci)]
-        L.rg_batch_dbg_size.argtypes = [vp]
-        L.rg_batch_scratch_bytes.argtypes = [vp]
-        L.rg_batch_destroy.argtypes = [vp]
-        L.rg_batch_bind.argtypes = [vp, ci, vp]
-        L.rg_batch_bind_param.argtypes = [vp, ctypes.c_char_p, vp]
-        L.rg_model_origin.argtypes = [vp, ctypes.POINTER(ctypes.c_float)]
-        L.rg_batch_launch_info.argtypes = [vp, ctypes.POINTER(ci), ctypes.POINTER(ci), ctypes.POINTER(ci)]
-        L.rg_batch_set_balance.argtypes = [vp, ci]
-        L.rg_step.argtypes = [vp, ci, ci, vp]
-        L.rg_step_subset.argtypes = [vp, vp, ci, ci, vp]
-        L.rg_forward.argtypes = [vp, vp]
-        L.rg_reset.argtypes = [vp, vp, vp]
-        L.rg_set_const.argtypes = [vp, vp, vp]
-        L.rg_batch_update_pairs.argtypes = [vp, vp, vp]
-        L.rg_batch_mark_pairs_stale.argtypes = [vp, vp, vp]
-        L.rg_batch_set_pair_capacity.argtypes = [vp, ci]
-        L.rg_batch_pair_info.argtypes = [vp, ctypes.POINTER(ci), ctypes.POINTER(vp)]
+        for name, (restype, argtypes) in SIGNATURES.items():
+            f = getattr(L, name)
+            f.restype, f.argtypes = restype, argtypes
         _lib = L
     return _lib
 
@@ -80,6 +130,38 @@ def lib():
 def _check(rc):
     if rc != 0:
         raise EngineError(lib().rg_last_error().decode())
+
+
+def ptr(x):
+    """The data pointer of a tensor as a pointer argument; None (NULL) for None."""
+    return None if x is None else ctypes.c_void_p(x.data_ptr())
+
+
+def current_stream(t, device):
+    """torch's current stream on `device` as the stream argument (cudaStream_t) of a launch."""
+    return ctypes.c_void_p(t.cuda.current_stream(device).cuda_stream)
+
+
+def as_device(t, x, dtype, shape, name, device):
+    """`x` (a tensor or anything numpy takes) broadcast to `shape` as a contiguous `dtype` tensor on `device`; ValueError
+    naming `name` when it does not broadcast."""
+    x = x if t.is_tensor(x) else t.as_tensor(np.asarray(x))
+    if tuple(x.shape) != tuple(shape):
+        try:
+            x = x.expand(*shape)
+        except RuntimeError:
+            raise ValueError(f"{name}: expected shape {tuple(shape)}, got {tuple(x.shape)}") from None
+    return x.to(device=device, dtype=dtype).contiguous()
+
+
+def device_mask(t, mask, nenv, device):
+    """A [nenv] environment mask (bool or uint8, tensor or array; None: every environment) as the contiguous uint8 tensor on
+    `device` that the launches read, or None.
+
+    Lifetime: the result, like every other temporary as_device makes for a launch, may be dropped as soon as the launch is
+    enqueued, with no synchronisation.  It is allocated on torch's current stream of `device`, the stream the launch is
+    enqueued on, and the caching allocator gives its memory only to later work on that stream, which runs after the launch."""
+    return None if mask is None else as_device(t, mask, t.uint8, (nenv,), "mask", device)
 
 
 def check_geom_dataid(v, m):
@@ -130,8 +212,8 @@ class DeviceModel:
             import sys
 
             t = sys.modules.get("torch")
-            stream = t.cuda.current_stream(self.device).cuda_stream if t is not None and t.cuda.is_available() else 0
-        _check(lib().rg_model_set_field_async(self.h, name.encode(), buf.ctypes.data, buf.size, ctypes.c_void_p(stream)))
+            stream = current_stream(t, self.device) if t is not None and t.cuda.is_available() else None
+        _check(lib().rg_model_set_field_async(self.h, name.encode(), buf.ctypes.data, buf.size, stream))
 
     def name2id(self, objtype, name):
         """mjModel.<objtype>_name2id through the C ABI (the blob carries its name tables)."""
@@ -242,7 +324,7 @@ class BatchedSim:
     def _bind(self, fid, t):
         assert t.is_contiguous()
         self._bound[fid] = t  # keep alive
-        _check(lib().rg_batch_bind(self.h, fid, ctypes.c_void_p(t.data_ptr())))
+        _check(lib().rg_batch_bind(self.h, fid, ptr(t)))
 
     def enable_xfrc(self):
         m = self.model.host
@@ -267,13 +349,11 @@ class BatchedSim:
                 raise EngineError(f"set_param(geom_dataid): expected {m['ngeom']} values per environment, got {v.shape[1]}")
             check_geom_dataid(v, m)
             out = self._store_param(name, v.to(device=self.device, dtype=t.int32).contiguous(), idx)
-            mp = None
+            mask = None
             if idx is not None:
-                mk = t.zeros(self.nenv, dtype=t.uint8, device=self.device)
-                mk[t.as_tensor(idx, device=self.device).long()] = 1
-                self._keep_stale = mk            # alive until the launch has consumed it
-                mp = ctypes.c_void_p(mk.data_ptr())
-            _check(lib().rg_batch_mark_pairs_stale(self.h, mp, self._stream()))
+                mask = t.zeros(self.nenv, dtype=t.uint8, device=self.device)
+                mask[t.as_tensor(idx, device=self.device).long()] = 1
+            _check(lib().rg_batch_mark_pairs_stale(self.h, ptr(mask), current_stream(t, self.device)))
             return out
         v = t.as_tensor(np.asarray(values, dtype=np.float64) if not t.is_tensor(values) else values).to(t.float64).reshape(rows, -1).clone()
         # mesh_scale / geom_mesh_scale: the engine's per-hull / per-mesh-geom scales, not blob arrays
@@ -300,18 +380,14 @@ class BatchedSim:
             self._params[name].copy_(dev)
         else:
             self._params[name] = dev
-            _check(lib().rg_batch_bind_param(self.h, name.encode(), ctypes.c_void_p(dev.data_ptr())))
+            _check(lib().rg_batch_bind_param(self.h, name.encode(), ptr(dev)))
         return self._params[name]
 
     def update_pairs(self, mask=None):
         """Rederive the per-environment pair lists from the bound geom_dataid rows (all environments, or those of `mask`):
         each keeps the static candidate pairs whose two geoms are enabled in its row (include/robogym_b200.h)."""
-        mp = None
-        if mask is not None:
-            mask = mask.to(device=self.device, dtype=self.torch.uint8).contiguous()
-            mp = ctypes.c_void_p(mask.data_ptr())
-            self._keep_mask = mask
-        _check(lib().rg_batch_update_pairs(self.h, mp, self._stream()))
+        mask = device_mask(self.torch, mask, self.nenv, self.device)
+        _check(lib().rg_batch_update_pairs(self.h, ptr(mask), current_stream(self.torch, self.device)))
 
     def set_pair_capacity(self, capacity):
         """Pairs each environment's list can hold (0: npair); the lists are derived again before the next step."""
@@ -320,11 +396,11 @@ class BatchedSim:
     def pair_counts(self):
         """Length of every environment's pair list ([nenv] int32 device tensor, a copy), or None when the batch streams the
         static list."""
-        cap, ptr = ctypes.c_int(), ctypes.c_void_p()
-        _check(lib().rg_batch_pair_info(self.h, ctypes.byref(cap), ctypes.byref(ptr)))
-        if not ptr.value:
+        cap, counts = ctypes.c_int(), ctypes.c_void_p()
+        _check(lib().rg_batch_pair_info(self.h, ctypes.byref(cap), ctypes.byref(counts)))
+        if not counts.value:
             return None
-        view = type("EngineInts", (), {"__cuda_array_interface__": dict(shape=(self.nenv,), typestr="<i4", data=(ptr.value, False), version=2)})()
+        view = type("EngineInts", (), {"__cuda_array_interface__": dict(shape=(self.nenv,), typestr="<i4", data=(counts.value, False), version=2)})()
         return self.torch.as_tensor(view, device=self.device).clone()
 
     def enable_per_env_timestep(self):
@@ -332,33 +408,27 @@ class BatchedSim:
         self._bind(TIMESTEP, self.timestep)
         return self.timestep
 
-    def _stream(self):
-        return ctypes.c_void_p(self.torch.cuda.current_stream(self.device).cuda_stream)
-
     def step(self, n_substeps=None, final_forward=True, mask=None):
         """SimulationInterface.step(): nsubsteps x mj_step then mj_forward, for every environment (or, with `mask`
         -- a [nenv] bool/uint8 device tensor -- only for the selected ones; the launch then covers just those).
         final_forward may be an integer > 1 to fuse the extra sim.forward() calls of the reference's observation path."""
         nsub = self.n_substeps if n_substeps is None else int(n_substeps)
+        stream = current_stream(self.torch, self.device)
         if mask is None:
-            _check(lib().rg_step(self.h, nsub, int(final_forward), self._stream()))
+            _check(lib().rg_step(self.h, nsub, int(final_forward), stream))
         else:
-            mk = mask.to(device=self.device, dtype=self.torch.uint8).contiguous()
-            _check(lib().rg_step_subset(self.h, ctypes.c_void_p(mk.data_ptr()), nsub, int(final_forward), self._stream()))
-            self._keep_mask = mk   # alive until the launch has consumed it
+            mask = device_mask(self.torch, mask, self.nenv, self.device)
+            _check(lib().rg_step_subset(self.h, ptr(mask), nsub, int(final_forward), stream))
 
     def forward(self, mask=None, count=1):
         if mask is None and count == 1:
-            _check(lib().rg_forward(self.h, self._stream()))
+            _check(lib().rg_forward(self.h, current_stream(self.torch, self.device)))
         else:
             self.step(0, count, mask)
 
     def reset(self, mask=None):
-        mp = None
-        if mask is not None:
-            mask = mask.to(device=self.device, dtype=self.torch.uint8).contiguous()
-            mp = ctypes.c_void_p(mask.data_ptr())
-        _check(lib().rg_reset(self.h, mp, self._stream()))
+        mask = device_mask(self.torch, mask, self.nenv, self.device)
+        _check(lib().rg_reset(self.h, ptr(mask), current_stream(self.torch, self.device)))
 
     SET_CONST_FIELDS = ("dof_invweight0", "body_invweight0", "tendon_invweight0", "tendon_length0", "body_subtreemass", "opt_meaninertia")
 
@@ -372,12 +442,8 @@ class BatchedSim:
                 raise EngineError(f"set_const: {name} is not a constant mj_setConst derives")
             if name not in getattr(self, "_params", {}) and m[name].size:
                 self.set_param(name, np.repeat(np.asarray(m[name], dtype=np.float64).reshape(1, -1), self.nenv, axis=0))
-        mp = None
-        if mask is not None:
-            mask = mask.to(device=self.device, dtype=self.torch.uint8).contiguous()
-            mp = ctypes.c_void_p(mask.data_ptr())
-            self._keep_mask = mask
-        _check(lib().rg_set_const(self.h, mp, self._stream()))
+        mask = device_mask(self.torch, mask, self.nenv, self.device)
+        _check(lib().rg_set_const(self.h, ptr(mask), current_stream(self.torch, self.device)))
         return {k: self._params[k] for k in fields if k in self._params}
 
     def set_balance(self, on):

@@ -23,7 +23,7 @@ import ctypes
 import numpy as np
 
 from . import engine
-from .rearrange_placement import _dev
+from .engine import GoalIn, GoalOut, as_device, current_stream, device_mask, ptr
 
 ROT_DIST = {"full": 0, "mod90": 1, "mod180": 2}
 ROT_RANDOMIZE = {"z_axis": 1, "block": 2}
@@ -31,42 +31,6 @@ SUCCESS_KEYS = {"obj_pos": 1, "obj_rot": 2}
 # envs/rearrange/common/base.py:130-137
 SUCCESS_THRESHOLD = {"obj_pos": 0.04, "obj_rot": 0.2}
 MAX_OBJECTS = 64
-
-_vp, _ci, _cd, _cll = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_longlong
-
-
-class GoalIn(ctypes.Structure):
-    """rg_goal_in (include/robogym_b200.h)"""
-    _fields_ = [("nenv", _ci), ("nobj", _ci), ("pos", _vp), ("quat", _vp), ("pos_stride", _cll), ("quat_stride", _cll), ("rows", _vp),
-                ("goal_pos", _vp), ("goal_quat", _vp), ("group", _vp), ("pos_offset", _vp), ("rot_weight", _vp), ("table", _cd * 6),
-                ("rot_dist_type", _ci), ("success_keys", _ci), ("pos_threshold", _cd), ("rot_threshold", _cd), ("reward_per_object", _cd)]
-
-
-class GoalOut(ctypes.Structure):
-    """rg_goal_out (include/robogym_b200.h)"""
-    _fields_ = [("obj_rot", _vp), ("rel_pos", _vp), ("rel_rot", _vp), ("dist_pos", _vp), ("dist_rot", _vp), ("success", _vp), ("off_table", _vp),
-                ("num_success", _vp), ("reward", _vp), ("achieved", _vp), ("any_off", _vp), ("pick", _vp)]
-
-
-_sigs = False
-
-
-def _lib():
-    global _sigs
-    L = engine.lib()
-    if not _sigs:
-        L.rg_rearrange_goal.argtypes = [ctypes.POINTER(GoalIn), _vp, _vp, ctypes.POINTER(GoalOut), _vp]
-        L.rg_goal_orientations.argtypes = [_ci, _ci, _vp, _vp, _ci, ctypes.c_uint32, ctypes.c_uint32, _vp, _vp, _vp]
-        _sigs = True
-    return L
-
-
-def _ptr(x):
-    return None if x is None else ctypes.c_void_p(x.data_ptr())
-
-
-def _stream(t, dev):
-    return ctypes.c_void_p(t.cuda.current_stream(dev).cuda_stream)
 
 
 def _settings(rot_dist_type, success_threshold):
@@ -83,14 +47,14 @@ def _settings(rot_dist_type, success_threshold):
 
 
 def _per_env(t, x, nenv, name, dev):
-    v = _dev(t, x, t.float64, (nenv,), name, dev)
+    v = as_device(t, x, t.float64, (nenv,), name, dev)
     if not bool(t.isfinite(v).all()):
         raise ValueError(f"{name}: finite")
     return v
 
 
 def _groups(t, groups, nenv, nobj, dev):
-    g = _dev(t, groups, t.int64, (nenv, nobj), "groups", dev)
+    g = as_device(t, groups, t.int64, (nenv, nobj), "groups", dev)
     if bool(((g < -1) | (g >= nobj)).any()):
         raise ValueError(f"groups: ids in [-1, {nobj}) (-1: an inactive slot)")
     return g.to(t.int32).contiguous()
@@ -129,14 +93,14 @@ class _Evaluation:
                         objects_off_table=t.zeros(nenv, nobj, **b), num_success=t.zeros(nenv, **f64), reward=t.zeros(nenv, **f64),
                         goal_achieved=t.zeros(nenv, **b), done=t.zeros(nenv, **b), pick=t.zeros(nenv, nobj, dtype=t.int32, device=dev))
         o = self.out
-        self.cout = GoalOut(_ptr(o["obj_rot"]), _ptr(o["rel_goal_obj_pos"]), _ptr(o["rel_goal_obj_rot"]), _ptr(o["dist_obj_pos"]), _ptr(o["dist_obj_rot"]),
-                            _ptr(o["success"]), _ptr(o["objects_off_table"]), _ptr(o["num_success"]), _ptr(o["reward"]), _ptr(o["goal_achieved"]),
-                            _ptr(o["done"]), _ptr(o["pick"]))
+        self.cout = GoalOut(ptr(o["obj_rot"]), ptr(o["rel_goal_obj_pos"]), ptr(o["rel_goal_obj_rot"]), ptr(o["dist_obj_pos"]), ptr(o["dist_obj_rot"]),
+                            ptr(o["success"]), ptr(o["objects_off_table"]), ptr(o["num_success"]), ptr(o["reward"]), ptr(o["goal_achieved"]),
+                            ptr(o["done"]), ptr(o["pick"]))
         self.cin = GoalIn()
         self.cin.nenv, self.cin.nobj = nenv, nobj
         self.cin.rows = self.rows.ctypes.data
-        self.cin.goal_pos, self.cin.goal_quat, self.cin.group = _ptr(self.goal_pos), _ptr(self.goal_quat), _ptr(self.groups)
-        self.cin.pos_offset, self.cin.rot_weight = _ptr(self.pos_offset), _ptr(self.rot_weight)
+        self.cin.goal_pos, self.cin.goal_quat, self.cin.group = ptr(self.goal_pos), ptr(self.goal_quat), ptr(self.groups)
+        self.cin.pos_offset, self.cin.rot_weight = ptr(self.pos_offset), ptr(self.rot_weight)
         self.cin.table[:] = _table(table).tolist()
         self.cin.rot_dist_type, self.cin.success_keys = rd, keys
         self.cin.pos_threshold, self.cin.rot_threshold, self.cin.reward_per_object = tp, tr, float(goal_reward_per_object)
@@ -145,14 +109,15 @@ class _Evaluation:
 
     def bind_poses(self, pos, quat, pos_stride, quat_stride):
         self._poses = (pos, quat)                        # alive while bound
-        self.cin.pos, self.cin.quat = _ptr(pos), _ptr(quat)
+        self.cin.pos, self.cin.quat = ptr(pos), ptr(quat)
         self.cin.pos_stride, self.cin.quat_stride = int(pos_stride), int(quat_stride)
 
     def run(self, mask=None):
         t = self.t
-        mk = None if mask is None else _dev(t, mask, t.uint8, (self.nenv,), "mask", self.dev)
+        mk = device_mask(t, mask, self.nenv, self.dev)
         with t.cuda.device(self.dev):
-            engine._check(_lib().rg_rearrange_goal(ctypes.byref(self.cin), _ptr(mk), _ptr(self.prev), ctypes.byref(self.cout), _stream(t, self.dev)))
+            engine._check(engine.lib().rg_rearrange_goal(ctypes.byref(self.cin), ptr(mk), ptr(self.prev), ctypes.byref(self.cout),
+                                                         current_stream(t, self.dev)))
         o = self.out
         return dict(rel_goal_obj_pos=o["rel_goal_obj_pos"], rel_goal_obj_rot=o["rel_goal_obj_rot"], goal_achieved=o["goal_achieved"],
                     goal_distance=dict(obj_pos=o["dist_obj_pos"], obj_rot=o["dist_obj_rot"]), success=o["success"], num_success=o["num_success"],
@@ -218,15 +183,15 @@ class BatchedRearrangeGoal:
         their previous success counts are cleared, so the next evaluation's reward is 0 (`_previous_goal_distance = None`).
         Returns goal_valid [nenv] bool: no active goal off the table (`next_goal`'s target_on_table)."""
         t, e, dev = self.t, self._e, self.sim.device
-        p = _dev(t, pos, t.float64, (self.nenv, self.nobj, 3), "pos", dev)
-        q = _dev(t, quat, t.float64, (self.nenv, self.nobj, 4), "quat", dev)
+        p = as_device(t, pos, t.float64, (self.nenv, self.nobj, 3), "pos", dev)
+        q = as_device(t, quat, t.float64, (self.nenv, self.nobj, 4), "quat", dev)
         if not bool(t.isfinite(p).all()):
             raise ValueError("pos: finite")
         _quat_ok(t, q, "quat")
         if mask is None:
             e.goal_pos.copy_(p); e.goal_quat.copy_(q); e.prev.fill_(float("nan"))
         else:
-            mk = _dev(t, mask, t.bool, (self.nenv,), "mask", dev)
+            mk = as_device(t, mask, t.bool, (self.nenv,), "mask", dev)
             e.goal_pos[mk] = p[mk]; e.goal_quat[mk] = q[mk]; e.prev[mk] = float("nan")
         return ~_objects_off_table(t, e.goal_pos, e.groups >= 0, self.table).any(dim=1)
 
@@ -257,10 +222,10 @@ def goal_distance(obj_pos, obj_quat, goal_pos, goal_quat, groups, table, rot_dis
     if not 1 <= nobj <= MAX_OBJECTS:
         raise ValueError(f"1 to {MAX_OBJECTS} objects per environment")
     dev = obj_pos.device
-    p = _dev(t, obj_pos, t.float32, (nenv, nobj, 3), "obj_pos", dev)
-    q = _dev(t, obj_quat, t.float32, (nenv, nobj, 4), "obj_quat", dev)
-    gp = _dev(t, goal_pos, t.float64, (nenv, nobj, 3), "goal_pos", dev)
-    gq = _dev(t, goal_quat, t.float64, (nenv, nobj, 4), "goal_quat", dev)
+    p = as_device(t, obj_pos, t.float32, (nenv, nobj, 3), "obj_pos", dev)
+    q = as_device(t, obj_quat, t.float32, (nenv, nobj, 4), "obj_quat", dev)
+    gp = as_device(t, goal_pos, t.float64, (nenv, nobj, 3), "goal_pos", dev)
+    gq = as_device(t, goal_quat, t.float64, (nenv, nobj, 4), "goal_quat", dev)
     if not bool(t.isfinite(p).all()) or not bool(t.isfinite(gp).all()):
         raise ValueError("positions: finite")
     _quat_ok(t, q, "obj_quat")
@@ -301,9 +266,9 @@ def goal_orientations(base_quat, active, seed, epoch, mode="z_axis", mask=None):
     dev = base_quat.device
     out = base_quat.to(t.float64).contiguous().clone()
     _quat_ok(t, out, "base_quat")
-    act = _dev(t, active, t.uint8, (nenv, nobj), "active", dev)
-    mk = None if mask is None else _dev(t, mask, t.uint8, (nenv,), "mask", dev)
+    act = as_device(t, active, t.uint8, (nenv, nobj), "active", dev)
+    mk = device_mask(t, mask, nenv, dev)
     with t.cuda.device(dev):
-        engine._check(_lib().rg_goal_orientations(nenv, nobj, _ptr(out), _ptr(act), ROT_RANDOMIZE[mode], int(seed), int(epoch), _ptr(mk), _ptr(out),
-                                                  _stream(t, dev)))
+        engine._check(engine.lib().rg_goal_orientations(nenv, nobj, ptr(out), ptr(act), ROT_RANDOMIZE[mode], int(seed), int(epoch), ptr(mk),
+                                                        ptr(out), current_stream(t, dev)))
     return out

@@ -24,9 +24,9 @@ import ctypes
 import numpy as np
 
 from . import engine, modelblob
+from .engine import ObsIn, ObsOut, as_device, current_stream, device_mask, ptr
 from .rearrange_contacts import GRIPPER_BODIES
-from .rearrange_goal import MAX_OBJECTS, _lib as _goal_lib, _ptr, _stream
-from .rearrange_placement import _dev
+from .rearrange_goal import MAX_OBJECTS
 
 # envs/rearrange/simulation/base.py:110-112; safety_stop has no default (penalty.get("safety_stop", 0.0))
 PENALTY = {"table_collision": 0.0, "wrist_collision": 0.0, "objects_off_table": 1.0, "safety_stop": 0.0}
@@ -34,44 +34,7 @@ GEOM_GRIPPER, GEOM_ROBOT = 1, 2
 WRIST_KEYS = ("table_collision_plane", "robot", "object", "any")
 OBJECT_KEYS = ("obj_pos", "obj_rot", "obj_rel_pos", "obj_vel_pos", "obj_vel_rot", "obj_gripper_contact", "obj_bbox_size", "obj_colors")
 GOAL_KEYS = ("goal_obj_pos", "goal_obj_rot", "rel_goal_obj_pos", "rel_goal_obj_rot")
-
-_vp, _ci, _cd = ctypes.c_void_p, ctypes.c_int, ctypes.c_double
-
-
-class ObsIn(ctypes.Structure):
-    """rg_obs_in (include/robogym_b200.h)"""
-    _fields_ = [("nenv", _ci), ("nobj", _ci), ("body_xpos", _vp), ("body_xquat", _vp), ("body_xvel", _vp), ("qpos", _vp), ("qvel", _vp),
-                ("ctrl", _vp), ("sensordata", _vp), ("contact", _vp), ("ncon", _vp), ("nbody", _ci), ("nq", _ci), ("nv", _ci), ("nu", _ci),
-                ("nsensordata", _ci), ("ncontact", _ci), ("ngeom", _ci), ("obj_body", _vp), ("obj_qpos", _vp), ("tcp_body", _ci),
-                ("narm", _ci), ("arm_qpos", _ci * 8), ("ngrip", _ci), ("grip_qpos", _ci * 4), ("grip_qvel", _ci * 4), ("grip_act", _ci),
-                ("force_adr", _ci), ("torque_adr", _ci), ("geom_object", _vp), ("geom_flags", _vp), ("table_plane", _ci), ("wrist_sphere", _ci),
-                ("pad", _ci * 2), ("goal_pos", _vp), ("goal_quat", _vp), ("rel_pos", _vp), ("rel_rot", _vp), ("achieved", _vp), ("off_table", _vp),
-                ("group", _vp), ("qpos_at_goal", _vp), ("bbox_size", _vp), ("colors", _vp), ("boundary", _vp), ("penalty", _cd * 4),
-                ("mask_obs", _ci), ("mask_margin", _cd)]
-
-
-OUT_FIELDS = ("obj_pos", "obj_rel_pos", "obj_vel_pos", "obj_rot", "obj_vel_rot", "robot_joint_pos", "gripper_pos", "gripper_velp", "gripper_controls",
-              "gripper_qpos", "gripper_vel", "qpos", "qpos_goal", "goal_obj_pos", "goal_obj_rot", "rel_goal_obj_pos", "rel_goal_obj_rot",
-              "is_goal_achieved", "obj_gripper_contact", "obj_bbox_size", "obj_colors", "safety_stop", "tcp_force", "tcp_torque", "placement_mask",
-              "goal_placement_mask") + tuple("masked_" + k for k in OBJECT_KEYS[:5]) + ("masked_obj_gripper_contact", "masked_obj_bbox_size",
-              "masked_obj_colors") + tuple("masked_" + k for k in GOAL_KEYS) + ("gripper_table_contact", "wrist_cam_contacts", "sim_reward", "sim_done")
-
-
-class ObsOut(ctypes.Structure):
-    """rg_obs_out (include/robogym_b200.h)"""
-    _fields_ = [(k, _vp) for k in OUT_FIELDS]
-
-
-_sigs = False
-
-
-def _lib():
-    global _sigs
-    L = _goal_lib()
-    if not _sigs:
-        L.rg_rearrange_obs.argtypes = [ctypes.POINTER(ObsIn), _vp, ctypes.POINTER(ObsOut), _vp]
-        _sigs = True
-    return L
+OUT_FIELDS = tuple(k for k, _ in ObsOut._fields_)
 
 
 def placement_area_boundary(table, area):
@@ -187,9 +150,9 @@ class BatchedRearrangeObservation:
 
         c = self.cin = ObsIn()
         c.nenv, c.nobj = nenv, nobj
-        c.body_xpos, c.body_xquat, c.body_xvel = _ptr(sim.body_xpos), _ptr(sim.body_xquat), _ptr(sim.body_xvel)
-        c.qpos, c.qvel, c.ctrl, c.sensordata = _ptr(sim.qpos), _ptr(sim.qvel), _ptr(sim.ctrl), _ptr(sim.sensordata)
-        c.contact, c.ncon = _ptr(sim.contact), _ptr(sim.ncon)
+        c.body_xpos, c.body_xquat, c.body_xvel = ptr(sim.body_xpos), ptr(sim.body_xquat), ptr(sim.body_xvel)
+        c.qpos, c.qvel, c.ctrl, c.sensordata = ptr(sim.qpos), ptr(sim.qvel), ptr(sim.ctrl), ptr(sim.sensordata)
+        c.contact, c.ncon = ptr(sim.contact), ptr(sim.ncon)
         c.nbody, c.nq, c.nv, c.nu, c.nsensordata, c.ncontact, c.ngeom = nbody, nq, int(m["nv"]), int(m["nu"]), int(m["nsensordata"]), int(sim.contact.shape[1]), ng
         c.obj_body, c.obj_qpos = self.obj_body.ctypes.data, self.obj_qpos.ctypes.data
         c.tcp_body, c.narm, c.ngrip, c.grip_act = T["tcp_body"], len(T["arm_qpos"]), len(T["grip_qpos"]), T["grip_act"]
@@ -197,15 +160,15 @@ class BatchedRearrangeObservation:
         c.grip_qpos[:c.ngrip] = T["grip_qpos"]
         c.grip_qvel[:c.ngrip] = T["grip_qvel"]
         c.force_adr, c.torque_adr = T["force_adr"], T["torque_adr"]
-        c.geom_object, c.geom_flags = _ptr(self.geom_object), _ptr(self.geom_flags)
+        c.geom_object, c.geom_flags = ptr(self.geom_object), ptr(self.geom_flags)
         c.table_plane, c.wrist_sphere = T["table_plane"], T["wrist_sphere"]
         c.pad[:] = T["pad"]
         e, go = goal._e, goal._e.out
-        c.goal_pos, c.goal_quat, c.group = _ptr(e.goal_pos), _ptr(e.goal_quat), _ptr(e.groups)
-        c.rel_pos, c.rel_rot = _ptr(go["rel_goal_obj_pos"]), _ptr(go["rel_goal_obj_rot"])
-        c.achieved, c.off_table = _ptr(go["goal_achieved"]), _ptr(go["objects_off_table"])
-        c.qpos_at_goal = _ptr(self.qpos_at_goal)
-        c.bbox_size, c.colors, c.boundary = _ptr(self.bbox_size), _ptr(self.colors), _ptr(self.boundary)
+        c.goal_pos, c.goal_quat, c.group = ptr(e.goal_pos), ptr(e.goal_quat), ptr(e.groups)
+        c.rel_pos, c.rel_rot = ptr(go["rel_goal_obj_pos"]), ptr(go["rel_goal_obj_rot"])
+        c.achieved, c.off_table = ptr(go["goal_achieved"]), ptr(go["objects_off_table"])
+        c.qpos_at_goal = ptr(self.qpos_at_goal)
+        c.bbox_size, c.colors, c.boundary = ptr(self.bbox_size), ptr(self.colors), ptr(self.boundary)
         c.penalty[:] = _penalty(penalty)
         c.mask_obs, c.mask_margin = int(self.mask_obs), float(mask_margin)
 
@@ -225,18 +188,18 @@ class BatchedRearrangeObservation:
         self.obs = o
         self.info = dict(gripper_table_contact=t.zeros(nenv, **b), wrist_cam_contacts=t.zeros(nenv, 4, **b), sim_reward=t.zeros(nenv, **f64),
                          sim_done=t.zeros(nenv, **b))
-        self.cout = ObsOut(**{k: _ptr(o.get(k, self.info.get(k))) for k in OUT_FIELDS})
+        self.cout = ObsOut(**{k: ptr(o.get(k, self.info.get(k))) for k in OUT_FIELDS})
 
     def set_reset_rows(self, bbox_size=None, colors=None, placement_area_boundary=None, mask=None):
         """Per-reset rows, for every environment or those of `mask` [nenv]: bbox_size [nenv, nobj, 3] (half sizes), colors
         [nenv, nobj, 4], placement_area_boundary [nenv, 6]; None keeps a row as it is."""
         t, dev, nenv, nobj = self.t, self.sim.device, self.nenv, self.nobj
-        mk = None if mask is None else _dev(t, mask, t.bool, (nenv,), "mask", dev)
+        mk = None if mask is None else as_device(t, mask, t.bool, (nenv,), "mask", dev)
         for x, dst, shape, name in ((bbox_size, self.bbox_size, (nenv, nobj, 3), "bbox_size"), (colors, self.colors, (nenv, nobj, 4), "colors"),
                                     (placement_area_boundary, self.boundary, (nenv, 6), "placement_area_boundary")):
             if x is None:
                 continue
-            v = _dev(t, x, t.float64, shape, name, dev)
+            v = as_device(t, x, t.float64, shape, name, dev)
             if not bool(t.isfinite(v).all()):
                 raise ValueError(f"{name}: finite")
             if mk is None:
@@ -248,11 +211,11 @@ class BatchedRearrangeObservation:
         """The qpos the goal was set on (next_goal copies the simulation's qpos into qpos_goal, object_state.py:381-390): `qpos`
         [nenv, nq] or None for the sim's current qpos, for every environment or those of `mask`.  Call it at every goal reset."""
         t, dev = self.t, self.sim.device
-        q = self.sim.qpos if qpos is None else _dev(t, qpos, t.float32, tuple(self.qpos_at_goal.shape), "qpos", dev)
+        q = self.sim.qpos if qpos is None else as_device(t, qpos, t.float32, tuple(self.qpos_at_goal.shape), "qpos", dev)
         if mask is None:
             self.qpos_at_goal.copy_(q)
         else:
-            mk = _dev(t, mask, t.bool, (self.nenv,), "mask", dev)
+            mk = as_device(t, mask, t.bool, (self.nenv,), "mask", dev)
             self.qpos_at_goal[mk] = q[mk]
 
     def observe(self, mask=None):
@@ -262,9 +225,9 @@ class BatchedRearrangeObservation:
         gripper_table_contact [nenv], wrist_cam_contacts [nenv, 4] (WRIST_KEYS), objects_off_table [nenv, nobj] (the goal's),
         sim_reward [nenv] (minus the penalties that apply) and sim_done [nenv] (an active object off the table)."""
         t = self.t
-        mk = None if mask is None else _dev(t, mask, t.uint8, (self.nenv,), "mask", self.sim.device)
+        mk = device_mask(t, mask, self.nenv, self.sim.device)
         with t.cuda.device(self.sim.device):
-            engine._check(_lib().rg_rearrange_obs(ctypes.byref(self.cin), _ptr(mk), ctypes.byref(self.cout), _stream(t, self.sim.device)))
+            engine._check(engine.lib().rg_rearrange_obs(ctypes.byref(self.cin), ptr(mk), ctypes.byref(self.cout), current_stream(t, self.sim.device)))
         info = dict(self.info)
         info["objects_off_table"] = self.goal._e.out["objects_off_table"]
         return self.obs, info

@@ -23,11 +23,10 @@ environments (objects, scales, yaws) and places them again under a mask.
     bbox = scene.bounding_boxes(quat)
     pos, status = object_placements(bbox, active, table, area, *seed.next())
 """
-import ctypes
-
 import numpy as np
 
 from . import engine, modelblob
+from .engine import as_device, current_stream, device_mask, ptr
 
 MODES = {"grid": 1, "uniform": 2, "goal_distance_ratio": 3, "grid_then_uniform": 4}
 STATUS = {0: None, 1: "grid", 2: "uniform", 3: "goal_distance_ratio"}
@@ -35,19 +34,6 @@ STATUS = {0: None, 1: "grid", 2: "uniform", 3: "goal_distance_ratio"}
 MAX_PLACEMENT_RETRY, MAX_PLACEMENT_RETRY_PER_OBJECT = 100, 20
 GOAL_DISTANCE_MIN = 0.06
 MAX_OBJECTS = 64
-
-_sigs = False
-
-
-def _lib():
-    global _sigs
-    L = engine.lib()
-    if not _sigs:
-        vp, ci, cd, u32 = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_uint32
-        L.rg_batch_body_aabb.argtypes = [vp, vp, ci, vp, vp, vp, vp]
-        L.rg_place_objects.argtypes = [ci, ci, vp, vp, vp, vp, ci, ci, ci, cd, cd, vp, u32, u32, vp, vp, vp, vp]
-        _sigs = True
-    return L
 
 
 def table_dimensions(model):
@@ -94,16 +80,6 @@ class PlacementSeed:
         return self.seed, e
 
 
-def _dev(t, x, dtype, shape, name, device):
-    x = x if t.is_tensor(x) else t.as_tensor(np.asarray(x))
-    if tuple(x.shape) != tuple(shape):
-        try:
-            x = x.expand(*shape)
-        except RuntimeError:
-            raise ValueError(f"{name}: expected shape {tuple(shape)}, got {tuple(x.shape)}") from None
-    return x.to(device=device, dtype=dtype).contiguous()
-
-
 def _place(bbox, active, table, area, seed, epoch, mode, mask, out, max_trials, max_per_object, anchor, ratio, dmin):
     import torch as t
 
@@ -120,8 +96,8 @@ def _place(bbox, active, table, area, seed, epoch, mode, mask, out, max_trials, 
     bb = bbox.to(t.float64).contiguous()
     if not bool(t.isfinite(bb).all()) or bool((bb[:, :, 1] < 0).any()):
         raise ValueError("bbox: finite, with half sizes >= 0")
-    act = _dev(t, active, t.uint8, (nenv, nobj), "active", dev)
-    ar = _dev(t, area, t.float64, (nenv, 6), "area", dev)
+    act = as_device(t, active, t.uint8, (nenv, nobj), "active", dev)
+    ar = as_device(t, area, t.float64, (nenv, 6), "area", dev)
     tab = np.concatenate([np.asarray(table[0], dtype=np.float64).reshape(3), np.asarray(table[1], dtype=np.float64).reshape(3)])
     if not (0 <= int(seed) < 1 << 32 and 0 <= int(epoch) < 1 << 32):
         raise ValueError("seed and epoch: 32-bit unsigned integers")
@@ -131,18 +107,16 @@ def _place(bbox, active, table, area, seed, epoch, mode, mask, out, max_trials, 
     if mode == "goal_distance_ratio":
         if anchor is None:
             raise ValueError("goal_distance_ratio: the object placements (anchor) are needed")
-        anc = _dev(t, anchor, t.float64, (nenv, nobj, 3), "anchor", dev)
-    mk = None if mask is None else _dev(t, mask, t.uint8, (nenv,), "mask", dev)
+        anc = as_device(t, anchor, t.float64, (nenv, nobj, 3), "anchor", dev)
+    mk = device_mask(t, mask, nenv, dev)
     pos = t.zeros(nenv, nobj, 3, dtype=t.float64, device=dev) if out is None else out
     if pos.dtype != t.float64 or tuple(pos.shape) != (nenv, nobj, 3) or not pos.is_contiguous() or pos.device != dev:
         raise ValueError("out: a contiguous float64 tensor [nenv, nobj, 3] on the device of bbox")
     status = t.full((nenv,), -1, dtype=t.int32, device=dev)
-    p = lambda x: None if x is None else ctypes.c_void_p(x.data_ptr())
     with t.cuda.device(dev):
-        stream = ctypes.c_void_p(t.cuda.current_stream(dev).cuda_stream)
-        engine._check(_lib().rg_place_objects(nenv, nobj, p(bb), p(act), tab.ctypes.data, p(ar), MODES[mode], int(max_trials), int(max_per_object),
-                                              float(ratio), float(dmin), p(anc), int(seed), int(epoch), p(mk), p(pos), p(status), stream))
-    # (the temporaries may be freed at once: the caching allocator reuses their memory only behind the launch on this stream)
+        engine._check(engine.lib().rg_place_objects(nenv, nobj, ptr(bb), ptr(act), tab.ctypes.data, ptr(ar), MODES[mode], int(max_trials),
+                                                    int(max_per_object), float(ratio), float(dmin), ptr(anc), int(seed), int(epoch), ptr(mk),
+                                                    ptr(pos), ptr(status), current_stream(t, dev)))
     return pos, status
 
 
@@ -179,11 +153,10 @@ def body_aabb(sim, bodies, quat=None, mask=None):
     n = len(bodies)
     if quat is None:
         quat = t.tensor([1.0, 0.0, 0.0, 0.0], dtype=t.float64)
-    q = _dev(t, quat, t.float64, (sim.nenv, n, 4), "quat", sim.device)
+    q = as_device(t, quat, t.float64, (sim.nenv, n, 4), "quat", sim.device)
     if not bool(t.isfinite(q).all()) or bool((q.norm(dim=2) == 0).any()):
         raise ValueError("quat: finite and non-zero")
-    mk = None if mask is None else _dev(t, mask, t.uint8, (sim.nenv,), "mask", sim.device)
+    mk = device_mask(t, mask, sim.nenv, sim.device)
     out = t.zeros(sim.nenv, n, 2, 3, dtype=t.float64, device=sim.device)
-    engine._check(_lib().rg_batch_body_aabb(sim.h, bodies.ctypes.data, n, ctypes.c_void_p(q.data_ptr()), None if mk is None else ctypes.c_void_p(mk.data_ptr()),
-                                            ctypes.c_void_p(out.data_ptr()), sim._stream()))
+    engine._check(engine.lib().rg_batch_body_aabb(sim.h, bodies.ctypes.data, n, ptr(q), ptr(mk), ptr(out), current_stream(t, sim.device)))
     return out

@@ -6,8 +6,7 @@ import subprocess
 
 import numpy as np
 
-from robogym_b200 import rearrange_goal as rg
-from robogym_b200 import rearrange_obs as ro
+from robogym_b200 import engine
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ENV_LIB = os.environ.get("RG_EMU_LIB")
@@ -58,12 +57,12 @@ def lib():
         L.rge_body_aabb.argtypes = [vp, ci, vp, vp, vp, vp, vp, vp, vp, vp]
         L.rge_place.argtypes = [ci, ci, vp, vp, vp, vp, ci, ci, ci, cd, cd, vp, u32, u32, vp, vp, vp]
         # goal evaluation and goal orientations
-        L.rge_goal.argtypes = [ctypes.POINTER(rg.GoalIn), vp, vp, ctypes.POINTER(rg.GoalOut)]
+        L.rge_goal.argtypes = [ctypes.POINTER(engine.GoalIn), vp, vp, ctypes.POINTER(engine.GoalOut)]
         L.rge_goal_error.restype = ctypes.c_char_p
         L.rge_goal_rot.argtypes = [ci, ci, vp, vp, ci, u32, u32, vp, vp]
         L.rge_parallel_quats.argtypes = [vp]
         # rearrange observations
-        L.rge_obs.argtypes = [ctypes.POINTER(ro.ObsIn), vp, ctypes.POINTER(ro.ObsOut)]
+        L.rge_obs.argtypes = [ctypes.POINTER(engine.ObsIn), vp, ctypes.POINTER(engine.ObsOut)]
         L.rge_obs_error.restype = ctypes.c_char_p
         _lib = L
     return _lib

@@ -1,23 +1,89 @@
-"""The C-ABI library exports every symbol include/robogym_b200.h declares (no compute calls, no GPU)."""
+"""The C ABI of include/robogym_b200.h: the library exports every function it declares, and the Python binding
+(robogym_b200.engine) declares the same functions, struct layouts and constants (no compute calls, no GPU)."""
 import ctypes
 import os
 import re
+import subprocess
 
 import pytest
 
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
+# the header's structs and their ctypes mirrors in robogym_b200.engine
+MIRRORS = {"rg_goal_in": "GoalIn", "rg_goal_out": "GoalOut", "rg_obs_in": "ObsIn", "rg_obs_out": "ObsOut"}
+
+
+def header():
+    """include/robogym_b200.h without its comments"""
+    return re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "robogym_b200.h")).read(), flags=re.S)
 
 
 def declared_functions():
-    src = open(os.path.join(ROOT, "include", "robogym_b200.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(rg_[a-z_]+)\s*\(", src)))
+    """{name: (return type, [parameter declarations])} of every function the header declares"""
+    out = {}
+    for ret, name, params in re.findall(r"^[ \t]*((?:const[ \t]+)?\w+[ \t]*\**)[ \t]*\b(rg_\w+)[ \t]*\(([^()]*)\)[ \t]*;", header(), re.M):
+        params = [" ".join(p.split()) for p in params.split(",")]
+        out[name] = (ret.strip(), [] if params == ["void"] else params)
+    return out
+
+
+def ctype_matches(decl, ct):
+    """whether the ctypes type `ct` passes the C type of `decl` (a return type, or a parameter's type and name): a pointer or
+    array as c_void_p or POINTER(...), a const char* as c_char_p, void as None and a scalar as its own ctypes type"""
+    if re.fullmatch(r"(const )?char ?\* ?\w*", decl):
+        return ct is ctypes.c_char_p
+    if "*" in decl or "[" in decl:
+        return ct is ctypes.c_void_p or (isinstance(ct, type) and issubclass(ct, ctypes._Pointer))
+    scalar = {"void": None, "int": ctypes.c_int, "size_t": ctypes.c_size_t, "double": ctypes.c_double, "uint32_t": ctypes.c_uint32}
+    return ct is scalar[decl.split()[0]]
 
 
 def test_header_declares_the_boundary():
     fns = declared_functions()
     for f in ("rg_model_load", "rg_batch_create", "rg_batch_bind", "rg_step", "rg_forward", "rg_reset", "rg_last_error"):
         assert f in fns
+
+
+def test_signature_table_matches_the_header():
+    """engine.SIGNATURES covers exactly the functions the header declares, each with its arity and, for the return value and
+    every parameter, a ctypes type of the declared kind."""
+    from robogym_b200 import engine
+
+    decl = declared_functions()
+    assert sorted(engine.SIGNATURES) == sorted(decl)
+    for name, (ret, params) in decl.items():
+        restype, argtypes = engine.SIGNATURES[name]
+        assert len(argtypes) == len(params), f"{name}: {len(argtypes)} argtypes for {len(params)} parameters"
+        assert ctype_matches(ret, restype), f"{name}: restype {restype} for {ret}"
+        for i, (p, ct) in enumerate(zip(params, argtypes)):
+            assert ctype_matches(p, ct), f"{name}: argument {i} ({p}) declared as {ct}"
+
+
+def test_struct_mirrors_and_constants_match_the_header(tmp_path):
+    """A C program built from the header by the host compiler prints sizeof of every mirrored struct, offsetof and sizeof of
+    each field the ctypes mirrors declare, every rg_field enumerator and RG_MAX_CONTACTS; ctypes and engine's constants
+    must give the same numbers."""
+    from robogym_b200 import engine
+
+    lines, expect = [], {}
+    for cname, pyname in MIRRORS.items():
+        mirror = getattr(engine, pyname)
+        lines.append(f'printf("sizeof {cname} %zu\\n", sizeof({cname}));')
+        expect[f"sizeof {cname}"] = ctypes.sizeof(mirror)
+        for f, _ in mirror._fields_:
+            lines.append(f'printf("offsetof {cname}.{f} %zu\\n", offsetof({cname}, {f}));')
+            lines.append(f'printf("sizeof {cname}.{f} %zu\\n", sizeof((({cname}*)0)->{f}));')
+            expect[f"offsetof {cname}.{f}"], expect[f"sizeof {cname}.{f}"] = getattr(mirror, f).offset, getattr(mirror, f).size
+    fields = re.findall(r"\b(RG_FIELD_\w+)\s*=", header())
+    for e in fields + ["RG_MAX_CONTACTS"]:
+        lines.append(f'printf("{e} %d\\n", (int){e});')
+    expect.update({e: getattr(engine, e[len("RG_FIELD_"):]) for e in fields})
+    expect["RG_MAX_CONTACTS"] = engine.MAX_CONTACTS
+    src, exe = tmp_path / "abi_layout.c", tmp_path / "abi_layout"
+    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "robogym_b200.h"\nint main(void) {\n' + "\n".join(lines) + "\nreturn 0;\n}\n")
+    subprocess.run([os.environ.get("CC", "cc"), "-std=c11", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
+    out = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout
+    got = {k: int(v) for k, v in (line.rsplit(" ", 1) for line in out.splitlines())}
+    assert got == expect
 
 
 def test_library_exports_every_declared_symbol():

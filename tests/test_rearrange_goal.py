@@ -17,6 +17,7 @@ import pytest
 
 import pyemu
 from goal_rng import GoalRotReplayRandomState
+from robogym_b200 import engine
 from robogym_b200 import rearrange_goal as rg
 
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
@@ -45,7 +46,7 @@ class EmuGoal:
                         success=z(nenv, nobj, d=np.uint8), off_table=z(nenv, nobj, d=np.uint8), num_success=z(nenv), reward=z(nenv),
                         achieved=z(nenv, d=np.uint8), any_off=z(nenv, d=np.uint8), pick=z(nenv, nobj, d=np.int32))
         o = self.out
-        self.cout = rg.GoalOut(*[_p(o[k]) for k in ("obj_rot", "rel_pos", "rel_rot", "dist_pos", "dist_rot", "success", "off_table", "num_success",
+        self.cout = engine.GoalOut(*[_p(o[k]) for k in ("obj_rot", "rel_pos", "rel_rot", "dist_pos", "dist_rot", "success", "off_table", "num_success",
                                                     "reward", "achieved", "any_off", "pick")])
         self.mode, self.table, self.threshold, self.reward_per_object = mode, np.asarray(table, dtype=np.float64), threshold, reward_per_object
 
@@ -59,7 +60,7 @@ class EmuGoal:
                     w=np.ascontiguousarray(np.broadcast_to(weight, (n,)), dtype=np.float64),
                     rows=np.ascontiguousarray(np.arange(k) if rows is None else rows, dtype=np.int32),
                     mask=None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8))
-        ci = rg.GoalIn()
+        ci = engine.GoalIn()
         ci.nenv, ci.nobj = n, k
         ci.pos, ci.quat = _p(keep["pos"]), _p(keep["quat"])
         ci.pos_stride, ci.quat_stride = (3 * k, 4 * k) if stride is None else stride

@@ -15,6 +15,7 @@ import numpy as np
 import pytest
 
 import pyemu
+from robogym_b200 import engine
 from robogym_b200 import rearrange_goal as rg
 from robogym_b200 import rearrange_obs as ro
 
@@ -55,10 +56,10 @@ class EmuObs:
             self.out.update(placement_mask=z(n, k, 1), goal_placement_mask=z(n, k, 1))
             for key in ro.OBJECT_KEYS + ro.GOAL_KEYS:
                 self.out["masked_" + key] = np.zeros_like(self.out[key])
-        self.cout = ro.ObsOut(**{f: _p(self.out.get(f)) for f in ro.OUT_FIELDS})
+        self.cout = engine.ObsOut(**{f: _p(self.out.get(f)) for f in ro.OUT_FIELDS})
         self.keep = dict(obj_body=np.asarray(T["obj_body"], np.int32), obj_qpos=np.asarray(T["obj_qpos"], np.int32),
                          geom_object=np.asarray(T["geom_object"], np.int32), geom_flags=np.asarray(T["geom_flags"], np.uint8))
-        c = self.cin = ro.ObsIn()
+        c = self.cin = engine.ObsIn()
         c.nenv, c.nobj = n, k
         c.nbody, c.nq, c.nv, c.nu, c.nsensordata, c.ngeom = T["nbody"], T["nq"], T["nv"], T["nu"], T["nsensordata"], T["ngeom"]
         c.obj_body, c.obj_qpos = _p(self.keep["obj_body"]), _p(self.keep["obj_qpos"])
