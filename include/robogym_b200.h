@@ -209,6 +209,28 @@ int rg_batch_body_aabb(rg_batch* b, const int* bodies, int nsel, const double* q
 int rg_place_objects(int nenv, int nobj, const double* bbox, const uint8_t* active, const double table[6], const double* area, int mode,
                      int max_trials, int max_per_object, double goal_distance_ratio, double goal_distance_min, const double* anchor,
                      uint32_t seed, uint32_t epoch, const uint8_t* mask_device, double* pos, int* status, void* stream);
+/* The reference's other goal generators as edits of a placement, after rg_place_objects on the same stream, one thread per
+ * selected environment (mask as above).  pos [nenv][nobj][3] (device, fp64) is edited in place on the active slots (uint8
+ * [nenv][nobj], the reference's objects in slot order); inactive slots are not written.  kind:
+ *   1 stack  (ObjectStackGoal._sample_next_goal_positions, goals/object_stack_goal.py): pos holds the bottom position in the
+ *            first active slot; the active objects are taken in block order (0..n-1 with fixed_order, else numpy's shuffle)
+ *            and object order[i] goes to the bottom position raised by i * object_size * 2;
+ *   2 lift   (move_one_object_to_the_air, goals/pickandplace.py): one active object, randint(n), raised by
+ *            uniform(min_height, max_height);
+ *   3 train  (move_one_object_to_the_air_with_restrictions, goals/train_state.py): p = random(); nothing when
+ *            p > pickup_proba + stacking_proba (or both are 0: no draw), a lift by the height times goal_distance_ratio when
+ *            p < pickup_proba, otherwise (n >= 2) a tower of randint(2, n + 1) distinct objects on the first one's xy, member
+ *            k + 1 raised by object_size * (k + 1) * 2.  The reference draws the members with the global np.random.choice;
+ *            here they come from a partial Fisher-Yates draw on the environment's own stream;
+ *   4 reach  (ObjectReachGoal._sample_next_goal_positions, goals/object_reach_goal.py): the one active object raised by
+ *            target_height (an environment with another count is left alone).
+ * object_size (stack, train), goal_distance_ratio (train) and target_height (reach) are fp64 [nenv] device arrays, NULL for
+ * the kinds that do not read them.  Random numbers: Philox4x32-10 keyed by (seed, environment), draw d of the modifier at
+ * counter (d, 0, 3, epoch) (robogym_b200/csrc/rg_place.inl lists d for every draw), so results do not depend on the mask.
+ * Asynchronous on `stream`, on the current device. */
+int rg_goal_modify(int nenv, int nobj, int kind, const uint8_t* active, const double* object_size, const double* goal_distance_ratio,
+                   const double* target_height, double min_height, double max_height, double pickup_proba, double stacking_proba, int fixed_order,
+                   uint32_t seed, uint32_t epoch, const uint8_t* mask_device, double* pos, void* stream);
 
 /* Rearrange goal evaluation, once per env-step: the reference's ObjectStateGoal.relative_goal / goal_distance
  * (robogym/envs/rearrange/goals/object_state.py:492-599), RearrangeEnv._calculate_num_success /
@@ -221,7 +243,12 @@ int rg_place_objects(int nenv, int nobj, const double* bbox, const uint8_t* acti
  *   goal_pos / goal_quat: fp64 [nenv][nobj][3|4]; group: int32 [nenv][nobj], the object's group id (duplicates share one),
  *     -1 for an inactive (padded) slot; pos_offset / rot_weight: fp64 [nenv] (goal_pos_offset, goal_rot_weight).
  *   table: table body pos, table geom half size (as rg_place_objects); rot_dist_type 0 full, 1 mod90, 2 mod180;
- *   success_keys: bit 0 obj_pos, bit 1 obj_rot in success_threshold (at least one), with their thresholds.
+ *   success_keys: bit 0 obj_pos, bit 1 obj_rot, bit 2 gripper_pos, bit 3 grasped in success_threshold (at least one), with
+ *     their thresholds.
+ *   Optional, at the end of the struct (NULL / 0: not read, and every other output is as without them), ObjectStackGoal's keys
+ *   (goals/object_stack_goal.py): gripper_pos, float32, read in place at gripper_pos[e * gripper_stride] (a BatchedSim's
+ *   site_xpos offset to the grip site's row, stride 3 * nsite); grasped, fp64 [nenv][nobj], the sum of the two pad contact
+ *   flags per slot (is_object_grasped).  Bit 2 needs gripper_pos, bit 3 grasped.
  * Semantics: object angles are normalize_angles(mat2euler(quat2mat(q))) (get_object_rot), goal angles mat2euler(quat2mat(q))
  * (get_target_rot); inactive slots are zero on both sides.  Within every group of two or more active slots objects are
  * matched to goals greedily (the first flat argmin of the position distances, repeated); the others keep their own goal.
@@ -229,7 +256,8 @@ int rg_place_objects(int nenv, int nobj, const double* bbox, const uint8_t* acti
  * evaluation's num_success; NaN marks "none since the goal reset" and gives reward 0.  Outputs per slot: obj_rot, rel_pos,
  * rel_rot ([nenv][nobj][3]), dist_pos, dist_rot ([nenv][nobj]), success, off_table (uint8 [nenv][nobj]); per environment:
  * num_success (count x reward_per_object), reward (num_success - prev), achieved, any_off (uint8).  pick (optional, int32
- * [nenv][nobj]): matched goal slot * 32 + index of the parallel quaternion taken (31: none).  fp64 with explicitly rounded
+ * [nenv][nobj]): matched goal slot * 32 + index of the parallel quaternion taken (31: none).  rel_gripper [nenv][nobj][3] and
+ * dist_gripper [nenv][nobj] (optional, with gripper_pos): obj_pos - gripper_pos and its norm, padded slots at -gripper_pos.  fp64 with explicitly rounded
  * operations in the reference's order (robogym_b200/csrc/rg_goal.inl).  Asynchronous on `stream`, on the current device. */
 typedef struct rg_goal_in {
   int nenv, nobj;
@@ -242,6 +270,9 @@ typedef struct rg_goal_in {
   double table[6];
   int rot_dist_type, success_keys;
   double pos_threshold, rot_threshold, reward_per_object;
+  const float* gripper_pos; long long gripper_stride;
+  const double* grasped;
+  double gripper_threshold, grasped_threshold;
 } rg_goal_in;
 typedef struct rg_goal_out {
   double* obj_rot; double* rel_pos; double* rel_rot;
@@ -250,6 +281,7 @@ typedef struct rg_goal_out {
   double* num_success; double* reward;
   uint8_t* achieved; uint8_t* any_off;
   int* pick;
+  double* rel_gripper; double* dist_gripper;
 } rg_goal_out;
 int rg_rearrange_goal(const rg_goal_in* in, const uint8_t* mask_device, double* prev, const rg_goal_out* out, void* stream);
 /* Goal orientations at goal reset: randomize_quaternion_along_z (mode 1: quat_mul(z_quat, base)) or randomize_quaternion_block

@@ -328,6 +328,12 @@ __global__ void __launch_bounds__(128) rg_place_kernel(const __grid_constant__ R
   if (env >= a.nenv || (a.mask && !a.mask[env])) return;
   rg_place_env(a, (uint32_t)env, threadIdx.x & 31);
 }
+/* rg_goal_modify: one thread per selected environment */
+__global__ void __launch_bounds__(128) rg_modify_kernel(const __grid_constant__ RgModifyArgs a) {
+  const int env = blockIdx.x * blockDim.x + threadIdx.x;
+  if (env >= a.nenv || (a.mask && !a.mask[env])) return;
+  rg_modify_env(a, (uint32_t)env);
+}
 /* rg_rearrange_goal: one warp per selected environment, its working set in shared memory */
 #define RG_GOAL_WARPS 4
 __global__ void __launch_bounds__(32 * RG_GOAL_WARPS) rg_goal_kernel(const __grid_constant__ RgGoalArgs a) {
@@ -936,6 +942,18 @@ int rg_place_objects(int nenv, int nobj, const double* bbox, const uint8_t* acti
   a.seed = seed; a.epoch = epoch;
   a.bbox = bbox; a.active = active; a.area = area; a.anchor = anchor; a.mask = mask; a.pos = pos; a.status = status;
   rg_place_kernel<<<(nenv + 3) / 4, 128, 0, (cudaStream_t)stream>>>(a);
+  RG_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rg_goal_modify(int nenv, int nobj, int kind, const uint8_t* active, const double* object_size, const double* goal_distance_ratio,
+                   const double* target_height, double min_height, double max_height, double pickup_proba, double stacking_proba, int fixed_order,
+                   uint32_t seed, uint32_t epoch, const uint8_t* mask, double* pos, void* stream) {
+  RgModifyArgs a;
+  const char* err = rg_modify_make_args(nenv, nobj, kind, active, object_size, goal_distance_ratio, target_height, min_height, max_height, pickup_proba,
+                                        stacking_proba, fixed_order, seed, epoch, mask, pos, a);
+  if (err) return rg_fail(-1, std::string("rg_goal_modify: ") + err);
+  rg_modify_kernel<<<(nenv + 127) / 128, 128, 0, (cudaStream_t)stream>>>(a);
   RG_CUDA(cudaGetLastError());
   return 0;
 }

@@ -31,13 +31,14 @@ class GoalIn(ctypes.Structure):
     """rg_goal_in (include/robogym_b200.h)"""
     _fields_ = [("nenv", _ci), ("nobj", _ci), ("pos", _vp), ("quat", _vp), ("pos_stride", ctypes.c_longlong), ("quat_stride", ctypes.c_longlong),
                 ("rows", _vp), ("goal_pos", _vp), ("goal_quat", _vp), ("group", _vp), ("pos_offset", _vp), ("rot_weight", _vp), ("table", _cd * 6),
-                ("rot_dist_type", _ci), ("success_keys", _ci), ("pos_threshold", _cd), ("rot_threshold", _cd), ("reward_per_object", _cd)]
+                ("rot_dist_type", _ci), ("success_keys", _ci), ("pos_threshold", _cd), ("rot_threshold", _cd), ("reward_per_object", _cd),
+                ("gripper_pos", _vp), ("gripper_stride", ctypes.c_longlong), ("grasped", _vp), ("gripper_threshold", _cd), ("grasped_threshold", _cd)]
 
 
 class GoalOut(ctypes.Structure):
     """rg_goal_out (include/robogym_b200.h)"""
     _fields_ = [("obj_rot", _vp), ("rel_pos", _vp), ("rel_rot", _vp), ("dist_pos", _vp), ("dist_rot", _vp), ("success", _vp), ("off_table", _vp),
-                ("num_success", _vp), ("reward", _vp), ("achieved", _vp), ("any_off", _vp), ("pick", _vp)]
+                ("num_success", _vp), ("reward", _vp), ("achieved", _vp), ("any_off", _vp), ("pick", _vp), ("rel_gripper", _vp), ("dist_gripper", _vp)]
 
 
 class ObsIn(ctypes.Structure):
@@ -97,6 +98,7 @@ SIGNATURES = {
     "rg_reset": (_ci, [_vp, _vp, _vp]),
     "rg_batch_body_aabb": (_ci, [_vp, _vp, _ci, _vp, _vp, _vp, _vp]),
     "rg_place_objects": (_ci, [_ci, _ci, _vp, _vp, _vp, _vp, _ci, _ci, _ci, _cd, _cd, _vp, _u32, _u32, _vp, _vp, _vp, _vp]),
+    "rg_goal_modify": (_ci, [_ci, _ci, _ci, _vp, _vp, _vp, _vp, _cd, _cd, _cd, _cd, _ci, _u32, _u32, _vp, _vp, _vp]),
     "rg_rearrange_goal": (_ci, [_P(GoalIn), _vp, _vp, _P(GoalOut), _vp]),
     "rg_goal_orientations": (_ci, [_ci, _ci, _vp, _vp, _ci, _u32, _u32, _vp, _vp, _vp]),
     "rg_rearrange_obs": (_ci, [_P(ObsIn), _vp, _P(ObsOut), _vp]),

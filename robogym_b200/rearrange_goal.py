@@ -10,6 +10,12 @@ robogym_b200/csrc/rg_goal.inl), reading the objects' poses in place from the sim
 `goal_orientations` samples the reference's `randomize_quaternion_along_z` / `randomize_quaternion_block` with the placement
 kernel's counter-based random numbers.
 
+ObjectStackGoal's extra keys (goals/object_stack_goal.py) come from the same launch when a gripper position is bound
+(`gripper_site`, or `gripper_pos` of goal_distance): goal_distance["gripper_pos"] is |obj_pos - gripper_pos| per slot,
+goal_distance["grasped"] the pad-contact sum passed to evaluate(), and both may appear in success_threshold.  With
+goal_pos_offset 0, goal_rot_weight 1 and distinct groups the other keys are ObjectStackGoal's too.  `achieved_site` evaluates
+ObjectReachGoal instead: the achieved position is that site's position, its rotation zero.
+
 Padded slots (group -1) are zero on both sides, so they come out at distance max(goal_pos_offset, 0) and count as successes,
 as in the reference: that is why the reward is a difference of success counts.
 
@@ -27,7 +33,7 @@ from .engine import GoalIn, GoalOut, as_device, current_stream, device_mask, ptr
 
 ROT_DIST = {"full": 0, "mod90": 1, "mod180": 2}
 ROT_RANDOMIZE = {"z_axis": 1, "block": 2}
-SUCCESS_KEYS = {"obj_pos": 1, "obj_rot": 2}
+SUCCESS_KEYS = {"obj_pos": 1, "obj_rot": 2, "gripper_pos": 4, "grasped": 8}
 # envs/rearrange/common/base.py:130-137
 SUCCESS_THRESHOLD = {"obj_pos": 0.04, "obj_rot": 0.2}
 MAX_OBJECTS = 64
@@ -106,22 +112,45 @@ class _Evaluation:
         self.cin.pos_threshold, self.cin.rot_threshold, self.cin.reward_per_object = tp, tr, float(goal_reward_per_object)
         if not np.isfinite(self.cin.reward_per_object):
             raise ValueError("goal_reward_per_object: finite")
+        thr = SUCCESS_THRESHOLD if success_threshold is None else success_threshold
+        self.cin.gripper_threshold, self.cin.grasped_threshold = float(thr.get("gripper_pos", 0.0)), float(thr.get("grasped", 0.0))
+        self.grasped = None
+
+    def bind_gripper(self, pos, stride):
+        """ObjectStackGoal's gripper position, float32, read in place: environment e's at pos[e * stride] (pos: a tensor whose
+        first element is environment 0's x, or (tensor, offset in floats))"""
+        t, f64 = self.t, dict(dtype=self.t.float64, device=self.dev)
+        base, off = pos if isinstance(pos, tuple) else (pos, 0)
+        self._grip = base                                # alive while bound
+        self.cin.gripper_pos = ctypes.c_void_p(base.data_ptr() + 4 * int(off))
+        self.cin.gripper_stride = int(stride)
+        o = self.out
+        o["rel_gripper_pos"], o["dist_gripper_pos"] = t.zeros(self.nenv, self.nobj, 3, **f64), t.zeros(self.nenv, self.nobj, **f64)
+        self.cout.rel_gripper, self.cout.dist_gripper = ptr(o["rel_gripper_pos"]), ptr(o["dist_gripper_pos"])
 
     def bind_poses(self, pos, quat, pos_stride, quat_stride):
         self._poses = (pos, quat)                        # alive while bound
         self.cin.pos, self.cin.quat = ptr(pos), ptr(quat)
         self.cin.pos_stride, self.cin.quat_stride = int(pos_stride), int(quat_stride)
 
-    def run(self, mask=None):
+    def run(self, mask=None, grasped=None):
         t = self.t
         mk = device_mask(t, mask, self.nenv, self.dev)
+        self.grasped = None if grasped is None else as_device(t, grasped, t.float64, (self.nenv, self.nobj), "grasped", self.dev)
+        self.cin.grasped = ptr(self.grasped)
         with t.cuda.device(self.dev):
             engine._check(engine.lib().rg_rearrange_goal(ctypes.byref(self.cin), ptr(mk), ptr(self.prev), ctypes.byref(self.cout),
                                                          current_stream(t, self.dev)))
         o = self.out
-        return dict(rel_goal_obj_pos=o["rel_goal_obj_pos"], rel_goal_obj_rot=o["rel_goal_obj_rot"], goal_achieved=o["goal_achieved"],
-                    goal_distance=dict(obj_pos=o["dist_obj_pos"], obj_rot=o["dist_obj_rot"]), success=o["success"], num_success=o["num_success"],
-                    obj_rot=o["obj_rot"], reward=o["reward"], objects_off_table=o["objects_off_table"], done=o["done"], pick=o["pick"])
+        r = dict(rel_goal_obj_pos=o["rel_goal_obj_pos"], rel_goal_obj_rot=o["rel_goal_obj_rot"], goal_achieved=o["goal_achieved"],
+                 goal_distance=dict(obj_pos=o["dist_obj_pos"], obj_rot=o["dist_obj_rot"]), success=o["success"], num_success=o["num_success"],
+                 obj_rot=o["obj_rot"], reward=o["reward"], objects_off_table=o["objects_off_table"], done=o["done"], pick=o["pick"])
+        if "rel_gripper_pos" in o:
+            r["rel_gripper_pos"] = o["rel_gripper_pos"]
+            r["goal_distance"]["gripper_pos"] = o["dist_gripper_pos"]
+        if self.grasped is not None:
+            r["goal_distance"]["grasped"] = self.grasped
+        return r
 
 
 def _objects_off_table(t, pos, active, table):
@@ -138,21 +167,43 @@ class BatchedRearrangeGoal:
     sim: a BatchedSim with the outputs body_xpos and body_xquat; object_bodies: the body id of each object slot (<= 64);
     groups: [nenv, nobj] (or [nobj]) group id per slot, duplicates sharing one, -1 for an inactive (padded) slot;
     table: rearrange_placement.table_dimensions(model).  rot_dist_type, success_threshold, goal_reward_per_object are the
-    reference's constants; goal_pos_offset and goal_rot_weight its randomisable simulation parameters, scalars or [nenv]."""
+    reference's constants; goal_pos_offset and goal_rot_weight its randomisable simulation parameters, scalars or [nenv].
+    gripper_site (a site name, e.g. "robot0:grip"; the sim needs the output site_xpos) adds ObjectStackGoal's gripper_pos key.
+    achieved_site evaluates ObjectReachGoal: one slot whose achieved position is that site's (site_xpos) and whose rotation is
+    zero; object_bodies is then not read (None)."""
 
     def __init__(self, sim, object_bodies, groups, table, rot_dist_type="full", success_threshold=None, goal_reward_per_object=1.0,
-                 goal_pos_offset=0.0, goal_rot_weight=1.0):
+                 goal_pos_offset=0.0, goal_rot_weight=1.0, gripper_site=None, achieved_site=None):
         t = sim.torch
-        if getattr(sim, "body_xpos", None) is None or getattr(sim, "body_xquat", None) is None:
-            raise ValueError("the sim needs the outputs body_xpos and body_xquat")
-        bodies = np.asarray(object_bodies, dtype=np.int64).reshape(-1)
-        nbody = int(sim.body_xpos.shape[1])
-        if not 1 <= len(bodies) <= MAX_OBJECTS or (bodies < 0).any() or (bodies >= nbody).any():
-            raise ValueError(f"object_bodies: 1 to {MAX_OBJECTS} body ids in [0, {nbody})")
-        self.sim, self.t, self.nenv, self.nobj, self.table = sim, t, sim.nenv, len(bodies), table
-        self._e = _Evaluation(t, sim.device, sim.nenv, len(bodies), bodies, table, rot_dist_type, success_threshold, goal_reward_per_object,
-                              goal_pos_offset, goal_rot_weight)
-        self._e.bind_poses(sim.body_xpos, sim.body_xquat, 3 * nbody, 4 * nbody)
+        sites = {}
+        for name in (gripper_site, achieved_site):
+            if name is not None:
+                if getattr(sim, "site_xpos", None) is None:
+                    raise ValueError("a gripper or achieved site needs the sim output site_xpos")
+                sites[name] = sim.model.name2id("site", name)
+        nsite = 0 if getattr(sim, "site_xpos", None) is None else int(sim.site_xpos.shape[1])
+        if achieved_site is not None:
+            sid = sites[achieved_site]
+            self.sim, self.t, self.nenv, self.nobj, self.table = sim, t, sim.nenv, 1, table
+            self._e = _Evaluation(t, sim.device, sim.nenv, 1, [sid], table, rot_dist_type, success_threshold, goal_reward_per_object,
+                                  goal_pos_offset, goal_rot_weight)
+            # the site's rotation is the identity: quaternion rows up to the site's id, all (1, 0, 0, 0)
+            self._identity = t.zeros(sim.nenv, sid + 1, 4, dtype=t.float32, device=sim.device)
+            self._identity[..., 0] = 1.0
+            self._e.bind_poses(sim.site_xpos, self._identity, 3 * nsite, 4 * (sid + 1))
+        else:
+            if getattr(sim, "body_xpos", None) is None or getattr(sim, "body_xquat", None) is None:
+                raise ValueError("the sim needs the outputs body_xpos and body_xquat")
+            bodies = np.asarray(object_bodies, dtype=np.int64).reshape(-1)
+            nbody = int(sim.body_xpos.shape[1])
+            if not 1 <= len(bodies) <= MAX_OBJECTS or (bodies < 0).any() or (bodies >= nbody).any():
+                raise ValueError(f"object_bodies: 1 to {MAX_OBJECTS} body ids in [0, {nbody})")
+            self.sim, self.t, self.nenv, self.nobj, self.table = sim, t, sim.nenv, len(bodies), table
+            self._e = _Evaluation(t, sim.device, sim.nenv, len(bodies), bodies, table, rot_dist_type, success_threshold, goal_reward_per_object,
+                                  goal_pos_offset, goal_rot_weight)
+            self._e.bind_poses(sim.body_xpos, sim.body_xquat, 3 * nbody, 4 * nbody)
+        if gripper_site is not None:
+            self._e.bind_gripper((sim.site_xpos, 3 * sites[gripper_site]), 3 * nsite)
         self.set_groups(groups)
 
     @property
@@ -195,23 +246,26 @@ class BatchedRearrangeGoal:
             e.goal_pos[mk] = p[mk]; e.goal_quat[mk] = q[mk]; e.prev[mk] = float("nan")
         return ~_objects_off_table(t, e.goal_pos, e.groups >= 0, self.table).any(dim=1)
 
-    def evaluate(self, mask=None):
+    def evaluate(self, mask=None, grasped=None):
         """The goal information of the current poses (after a step or forward), for every environment or those of `mask` (the
         others keep their previous values): a dict of device tensors, overwritten by the next call --
         rel_goal_obj_pos / rel_goal_obj_rot [nenv, nobj, 3] (relative_goal), goal_distance {obj_pos, obj_rot} [nenv, nobj],
         success [nenv, nobj], num_success [nenv] (count x goal_reward_per_object, padded slots included), goal_achieved
         [nenv], reward [nenv] (num_success minus the previous evaluation's; 0 on the first after set_goal), obj_rot
         [nenv, nobj, 3] (get_object_rot), objects_off_table [nenv, nobj], done [nenv] (any object off the table), pick
-        [nenv, nobj] (matched goal slot * 32 + parallel quaternion index, 31: none)."""
-        return self._e.run(mask)
+        [nenv, nobj] (matched goal slot * 32 + parallel quaternion index, 31: none).  With a gripper_site: rel_gripper_pos
+        [nenv, nobj, 3] (obj_pos - gripper_pos) and goal_distance["gripper_pos"] [nenv, nobj]; with `grasped` ([nenv, nobj], the
+        two pad contact flags summed per slot, as is_object_grasped): goal_distance["grasped"]."""
+        return self._e.run(mask, grasped)
 
 
 def goal_distance(obj_pos, obj_quat, goal_pos, goal_quat, groups, table, rot_dist_type="full", success_threshold=None, goal_reward_per_object=1.0,
-                  goal_pos_offset=0.0, goal_rot_weight=1.0, previous=None, mask=None):
+                  goal_pos_offset=0.0, goal_rot_weight=1.0, previous=None, mask=None, gripper_pos=None, grasped=None):
     """The evaluation of BatchedRearrangeGoal on poses given as tensors: obj_pos [nenv, nobj, 3], obj_quat [nenv, nobj, 4] (CUDA; read
     as float32, as a sim stores them), goal_pos / goal_quat (float64), groups [nenv, nobj].  `previous` ([nenv] float64 CUDA,
-    in / out) carries the success count from one call to the next (NaN: none; None: a fresh one, reward 0).  Returns the dict
-    of evaluate() (new tensors) and "previous"."""
+    in / out) carries the success count from one call to the next (NaN: none; None: a fresh one, reward 0).  gripper_pos
+    ([nenv, 3], read as float32) and grasped ([nenv, nobj]) add ObjectStackGoal's keys.  Returns the dict of evaluate() (new
+    tensors) and "previous"."""
     import torch as t
 
     if not t.is_tensor(obj_pos) or not obj_pos.is_cuda:
@@ -239,7 +293,12 @@ def goal_distance(obj_pos, obj_quat, goal_pos, goal_quat, groups, table, rot_dis
             raise ValueError("previous: a contiguous float64 tensor [nenv] on the device of obj_pos")
         e.prev = previous
     e.bind_poses(p, q, 3 * nobj, 4 * nobj)
-    out = e.run(mask)
+    if gripper_pos is not None:
+        g = as_device(t, gripper_pos, t.float32, (nenv, 3), "gripper_pos", dev)
+        if not bool(t.isfinite(g).all()):
+            raise ValueError("gripper_pos: finite")
+        e.bind_gripper(g, 3)
+    out = e.run(mask, grasped)
     out["previous"] = e.prev
     return out
 

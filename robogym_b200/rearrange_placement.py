@@ -13,6 +13,10 @@ semantics and defaults, draw for draw: for the same random numbers the positions
 random numbers are Philox4x32-10 keyed by (seed, environment) and addressed by an `epoch` per call, so a masked re-placement
 draws the same numbers for an environment as a full one; `PlacementSeed` hands out a fresh epoch for every call.
 
+The reference's other goal generators edit such a placement (`rg_goal_modify`, one thread per environment, same random-number
+scheme under its own purpose): `stack_goals` (ObjectStackGoal), `pick_and_place_goals` (PickAndPlaceGoal), `train_goals`
+(TrainStateGoal with pickup / stacking tasks) and `reach_goals` (ObjectReachGoal).
+
 An environment no algorithm could place comes back with status 0 (its active slots zeroed).  The reference raises
 `InvalidSimulationError` there and `safe_reset_env` rebuilds the whole scene; here the caller redraws the flagged
 environments (objects, scales, yaws) and places them again under a mask.
@@ -34,6 +38,9 @@ STATUS = {0: None, 1: "grid", 2: "uniform", 3: "goal_distance_ratio"}
 MAX_PLACEMENT_RETRY, MAX_PLACEMENT_RETRY_PER_OBJECT = 100, 20
 GOAL_DISTANCE_MIN = 0.06
 MAX_OBJECTS = 64
+MODIFY = {"stack": 1, "lift": 2, "train": 3, "reach": 4}
+# goals/pickandplace.py:15, goals/object_state.py GoalArgs.height_range
+HEIGHT_RANGE = (0.05, 0.25)
 
 
 def table_dimensions(model):
@@ -142,6 +149,128 @@ def goal_placements(bbox, active, table, area, seed, epoch, mode="goal_distance_
     if mode not in ("goal_distance_ratio", "grid_then_uniform"):
         raise ValueError('goal modes: "goal_distance_ratio" or "grid_then_uniform"')
     return _place(bbox, active, table, area, seed, epoch, mode, mask, out, max_trials, max_per_object, anchor, goal_distance_ratio, goal_distance_min)
+
+
+def _active_counts(t, active, mask, nenv, nobj, dev):
+    """the active mask as the launches read it, and each selected environment's active count ([nenv] int64 on the host)"""
+    act = as_device(t, active, t.uint8, (nenv, nobj), "active", dev)
+    n = act.sum(1).cpu().numpy().astype(np.int64)
+    if mask is not None:
+        n = np.where(np.asarray(as_device(t, mask, t.bool, (nenv,), "mask", "cpu")), n, -1)
+    return act, n
+
+
+def _modify(kind, pos, act, seed, epoch, mask, object_size=None, ratio=None, target_height=None, height_range=(0.0, 0.0), pickup=0.0,
+            stacking=0.0, fixed_order=True):
+    import torch as t
+
+    nenv, nobj, dev = int(pos.shape[0]), int(pos.shape[1]), pos.device
+    per = {}
+    for name, v in (("object_size", object_size), ("goal_distance_ratio", ratio), ("target_height", target_height)):
+        if v is not None:
+            per[name] = as_device(t, v, t.float64, (nenv,), name, dev)
+            if not bool(t.isfinite(per[name]).all()):
+                raise ValueError(f"{name}: finite")
+    mk = device_mask(t, mask, nenv, dev)
+    with t.cuda.device(dev):
+        engine._check(engine.lib().rg_goal_modify(nenv, nobj, MODIFY[kind], ptr(act), ptr(per.get("object_size")), ptr(per.get("goal_distance_ratio")),
+                                                  ptr(per.get("target_height")), float(height_range[0]), float(height_range[1]), float(pickup),
+                                                  float(stacking), int(bool(fixed_order)), int(seed), int(epoch), ptr(mk), ptr(pos),
+                                                  current_stream(t, dev)))
+    return pos
+
+
+def _height_range(height_range):
+    lo, hi = (float(x) for x in height_range)
+    if not (np.isfinite(lo) and np.isfinite(hi) and lo <= hi):
+        raise ValueError("height_range: finite (min, max) with min <= max")
+    return lo, hi
+
+
+def _bbox_shape(bbox):
+    import torch as t
+
+    if not t.is_tensor(bbox) or not bbox.is_cuda or bbox.dim() != 4:
+        raise ValueError("bbox: a CUDA tensor [nenv, nobj, 2, 3] (bounding_boxes)")
+    return int(bbox.shape[0]), int(bbox.shape[1]), bbox.device
+
+
+def stack_goals(bbox, active, table, area, seed, epoch, object_size, fixed_order=False, mask=None, out=None, max_trials=MAX_PLACEMENT_RETRY,
+                max_per_object=MAX_PLACEMENT_RETRY_PER_OBJECT):
+    """`ObjectStackGoal._sample_next_goal_positions` (goals/object_stack_goal.py): the first active object placed alone by
+    place_objects_with_no_constraint, then every active object on that spot in block order (slot order with fixed_order, else
+    a shuffle), object i of the order raised by i * object_size * 2.  object_size: [nenv] or a scalar (each environment's block
+    size).  Every selected environment needs two or more active objects.  Returns (pos, status) as goal_placements; status is
+    the bottom object's placement (2, or 0: the tower is built on zeros, as the reference's)."""
+    import torch as t
+
+    nenv, nobj, dev = _bbox_shape(bbox)
+    act, n = _active_counts(t, active, mask, nenv, nobj, dev)
+    if ((n >= 0) & (n < 2)).any():
+        raise ValueError("stack_goals: every selected environment needs two or more active objects")
+    first = t.zeros_like(act)
+    first[t.arange(nenv, device=dev), act.argmax(1)] = 1
+    first &= act
+    pos, status = _place(bbox, first, table, area, seed, epoch, "uniform", mask, out, max_trials, max_per_object, None, 1.0, GOAL_DISTANCE_MIN)
+    return _modify("stack", pos, act, seed, epoch, mask, object_size=object_size, fixed_order=fixed_order), status
+
+
+def pick_and_place_goals(bbox, active, table, area, seed, epoch, height_range=HEIGHT_RANGE, mask=None, out=None, max_trials=MAX_PLACEMENT_RETRY,
+                         max_per_object=MAX_PLACEMENT_RETRY_PER_OBJECT):
+    """`PickAndPlaceGoal._sample_next_goal_positions` (goals/pickandplace.py): ObjectStateGoal's goals (grid, then uniform), then
+    one active object, randint(n), lifted by uniform(*height_range).  Returns (pos, status) as goal_placements."""
+    import torch as t
+
+    hr = _height_range(height_range)
+    nenv, nobj, dev = _bbox_shape(bbox)
+    act, n = _active_counts(t, active, mask, nenv, nobj, dev)
+    if (n == 0).any():
+        raise ValueError("pick_and_place_goals: every selected environment needs an active object")
+    pos, status = _place(bbox, act, table, area, seed, epoch, "grid_then_uniform", mask, out, max_trials, max_per_object, None, 1.0, GOAL_DISTANCE_MIN)
+    return _modify("lift", pos, act, seed, epoch, mask, height_range=hr), status
+
+
+def train_goals(bbox, active, table, area, seed, epoch, anchor, goal_distance_ratio=1.0, pickup_proba=0.0, stacking_proba=0.0,
+                height_range=HEIGHT_RANGE, object_size=0.0254, goal_distance_min=GOAL_DISTANCE_MIN, mask=None, out=None,
+                max_trials=MAX_PLACEMENT_RETRY, max_per_object=MAX_PLACEMENT_RETRY_PER_OBJECT):
+    """`TrainStateGoal._sample_next_goal_positions` (goals/train_state.py): goals pulled toward the object placements `anchor`
+    (goal_placements' "goal_distance_ratio"), then `move_one_object_to_the_air_with_restrictions`: p = random(); nothing when
+    p > pickup_proba + stacking_proba, a lift of uniform(*height_range) * goal_distance_ratio when p < pickup_proba, otherwise a
+    tower of randint(2, n + 1) active objects on the first one's xy, member k + 1 raised by object_size * (k + 1) * 2 (an
+    environment with fewer than two active objects is left as placed).  The reference draws the tower's members with the global
+    np.random.choice; here they are a partial Fisher-Yates draw from the environment's own stream.  goal_distance_ratio: a
+    scalar (the placement takes one); object_size: [nenv] or a scalar.  Returns (pos, status) as goal_placements."""
+    import torch as t
+
+    hr = _height_range(height_range)
+    pickup, stacking = float(pickup_proba), float(stacking_proba)
+    if not (pickup >= 0.0 and stacking >= 0.0 and 0.0 <= pickup + stacking <= 1.0):
+        raise ValueError("pickup_proba and stacking_proba: >= 0, with pickup_proba + stacking_proba in [0, 1]")
+    nenv, nobj, dev = _bbox_shape(bbox)
+    act, n = _active_counts(t, active, mask, nenv, nobj, dev)
+    if pickup > 0.0 and (n == 0).any():
+        raise ValueError("train_goals: a pickup draw needs an active object in every selected environment")
+    pos, status = _place(bbox, act, table, area, seed, epoch, "goal_distance_ratio", mask, out, max_trials, max_per_object, anchor,
+                         goal_distance_ratio, goal_distance_min)
+    return _modify("train", pos, act, seed, epoch, mask, object_size=object_size, ratio=float(goal_distance_ratio), height_range=hr, pickup=pickup,
+                   stacking=stacking), status
+
+
+def reach_goals(bbox, active, table, area, seed, epoch, target_height, mask=None, out=None, max_trials=MAX_PLACEMENT_RETRY,
+                max_per_object=MAX_PLACEMENT_RETRY_PER_OBJECT):
+    """`ObjectReachGoal._sample_next_goal_positions` (goals/object_reach_goal.py): the one object placed by
+    place_objects_with_no_constraint, then the goal target_height ([nenv] or a scalar) above it.  Every selected environment
+    must have exactly one active object (the reference asserts num_objects == 1).  Returns (goal_pos, object_pos, status):
+    object_pos is the placement the reference writes into the object's joint (set_object_pos)."""
+    import torch as t
+
+    nenv, nobj, dev = _bbox_shape(bbox)
+    act, n = _active_counts(t, active, mask, nenv, nobj, dev)
+    if ((n >= 0) & (n != 1)).any():
+        raise ValueError("reach_goals: every selected environment needs exactly one active object")
+    pos, status = _place(bbox, act, table, area, seed, epoch, "uniform", mask, out, max_trials, max_per_object, None, 1.0, GOAL_DISTANCE_MIN)
+    obj = pos.clone()
+    return _modify("reach", pos, act, seed, epoch, mask, target_height=target_height), obj, status
 
 
 def body_aabb(sim, bodies, quat=None, mask=None):
