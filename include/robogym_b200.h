@@ -231,6 +231,28 @@ int rg_place_objects(int nenv, int nobj, const double* bbox, const uint8_t* acti
 int rg_goal_modify(int nenv, int nobj, int kind, const uint8_t* active, const double* object_size, const double* goal_distance_ratio,
                    const double* target_height, double min_height, double max_height, double pickup_proba, double stacking_proba, int fixed_order,
                    uint32_t seed, uint32_t epoch, const uint8_t* mask_device, double* pos, void* stream);
+/* The reference's layout goal generators, one warp per selected environment (mask as above), on the active slots (uint8
+ * [nenv][nobj], the reference's objects in slot order; inactive slots are not written).  kind:
+ *   1 domino   (DominoStateGoal, goals/dominos.py: _create_new_domino_position_and_rotation, _adjust_and_check_fit,
+ *              _sample_next_goal_positions): up to max_retry arcs, each an offset random() * pi and a step
+ *              random() * pi / 4 - pi / 8; domino i turned by i * step + (offset + step / 2) about z and laid along the arc's
+ *              cumulative cos / sin steps of object_size * distance_mul; the first arc whose turned boxes fit in the placement
+ *              area is moved to a uniform spot in it.  status 0 when none fits (positions zeroed, the last arc's rotations);
+ *   2 attached (AttachedBlockStateGoal, goals/attached_block_state.py): exactly 8 active blocks (another count: status 0) in the
+ *              reference's pattern of object_size cells, rows permuted, at a uniform origin; identity rotations;
+ *   3 fixed    (ObjectFixedStateGoal, goals/object_state_fixed.py): rel [nenv][nobj][2], each object's placement relative to
+ *              the placement area (values outside [0, 1] are taken as they are); identity rotations.
+ * Attached and fixed are place_targets_with_fixed_position (common/utils.py): the proposal and _get_global_placement of
+ * rg_place_objects, no collision or bounds check, status 1.  Device inputs: bbox [nenv][nobj][2][3] unrotated body boxes
+ * (rg_batch_body_aabb with the identity), area [nenv][6], object_size / distance_mul fp64 [nenv] (NULL for the kinds that do
+ * not read them); host: table as rg_place_objects.  Out (device): pos [nenv][nobj][3] fp64 body-origin positions, quat
+ * [nenv][nobj][4] fp64 (w x y z), status int32 [nenv] (1 placed, 0 not); optional (NULL: not written, domino only): angle fp64
+ * [nenv][nobj] the z angles, retry int32 [nenv] the arc that fitted (-1: none).  Random numbers: Philox4x32-10 keyed by (seed,
+ * environment), draw d at counter (d, 0, 4, epoch) (robogym_b200/csrc/rg_place.inl lists d for every draw), so results do not
+ * depend on the mask.  Asynchronous on `stream`, on the current device. */
+int rg_layout_goals(int nenv, int nobj, int kind, const double* bbox, const uint8_t* active, const double table[6], const double* area,
+                    const double* object_size, const double* distance_mul, const double* rel, int max_retry, uint32_t seed, uint32_t epoch,
+                    const uint8_t* mask_device, double* pos, double* quat, int* status, double* angle, int* retry, void* stream);
 
 /* Rearrange goal evaluation, once per env-step: the reference's ObjectStateGoal.relative_goal / goal_distance
  * (robogym/envs/rearrange/goals/object_state.py:492-599), RearrangeEnv._calculate_num_success /

@@ -334,6 +334,12 @@ __global__ void __launch_bounds__(128) rg_modify_kernel(const __grid_constant__ 
   if (env >= a.nenv || (a.mask && !a.mask[env])) return;
   rg_modify_env(a, (uint32_t)env);
 }
+/* rg_layout_goals: one warp per selected environment */
+__global__ void __launch_bounds__(128) rg_layout_kernel(const __grid_constant__ RgLayoutArgs a) {
+  const int env = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (env >= a.nenv || (a.mask && !a.mask[env])) return;
+  rg_layout_env(a, (uint32_t)env, threadIdx.x & 31);
+}
 /* rg_rearrange_goal: one warp per selected environment, its working set in shared memory */
 #define RG_GOAL_WARPS 4
 __global__ void __launch_bounds__(32 * RG_GOAL_WARPS) rg_goal_kernel(const __grid_constant__ RgGoalArgs a) {
@@ -954,6 +960,18 @@ int rg_goal_modify(int nenv, int nobj, int kind, const uint8_t* active, const do
                                         stacking_proba, fixed_order, seed, epoch, mask, pos, a);
   if (err) return rg_fail(-1, std::string("rg_goal_modify: ") + err);
   rg_modify_kernel<<<(nenv + 127) / 128, 128, 0, (cudaStream_t)stream>>>(a);
+  RG_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rg_layout_goals(int nenv, int nobj, int kind, const double* bbox, const uint8_t* active, const double table[6], const double* area,
+                    const double* object_size, const double* distance_mul, const double* rel, int max_retry, uint32_t seed, uint32_t epoch,
+                    const uint8_t* mask, double* pos, double* quat, int* status, double* angle, int* retry, void* stream) {
+  RgLayoutArgs a;
+  const char* err = rg_layout_make_args(nenv, nobj, kind, bbox, active, table, area, object_size, distance_mul, rel, max_retry, seed, epoch, mask, pos, quat,
+                                        status, angle, retry, a);
+  if (err) return rg_fail(-1, std::string("rg_layout_goals: ") + err);
+  rg_layout_kernel<<<(nenv + 3) / 4, 128, 0, (cudaStream_t)stream>>>(a);
   RG_CUDA(cudaGetLastError());
   return 0;
 }

@@ -99,6 +99,7 @@ SIGNATURES = {
     "rg_batch_body_aabb": (_ci, [_vp, _vp, _ci, _vp, _vp, _vp, _vp]),
     "rg_place_objects": (_ci, [_ci, _ci, _vp, _vp, _vp, _vp, _ci, _ci, _ci, _cd, _cd, _vp, _u32, _u32, _vp, _vp, _vp, _vp]),
     "rg_goal_modify": (_ci, [_ci, _ci, _ci, _vp, _vp, _vp, _vp, _cd, _cd, _cd, _cd, _ci, _u32, _u32, _vp, _vp, _vp]),
+    "rg_layout_goals": (_ci, [_ci, _ci, _ci, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ci, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rg_rearrange_goal": (_ci, [_P(GoalIn), _vp, _vp, _P(GoalOut), _vp]),
     "rg_goal_orientations": (_ci, [_ci, _ci, _vp, _vp, _ci, _u32, _u32, _vp, _vp, _vp]),
     "rg_rearrange_obs": (_ci, [_P(ObsIn), _vp, _P(ObsOut), _vp]),

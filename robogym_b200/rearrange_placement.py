@@ -15,7 +15,9 @@ draws the same numbers for an environment as a full one; `PlacementSeed` hands o
 
 The reference's other goal generators edit such a placement (`rg_goal_modify`, one thread per environment, same random-number
 scheme under its own purpose): `stack_goals` (ObjectStackGoal), `pick_and_place_goals` (PickAndPlaceGoal), `train_goals`
-(TrainStateGoal with pickup / stacking tasks) and `reach_goals` (ObjectReachGoal).
+(TrainStateGoal with pickup / stacking tasks) and `reach_goals` (ObjectReachGoal).  The generators that lay blocks out in a
+pattern compute goals and rotations from the boxes directly (`rg_layout_goals`, one warp per environment, its own purpose):
+`domino_goals` (DominoStateGoal), `attached_goals` (AttachedBlockStateGoal) and `fixed_goals` (ObjectFixedStateGoal).
 
 An environment no algorithm could place comes back with status 0 (its active slots zeroed).  The reference raises
 `InvalidSimulationError` there and `safe_reset_env` rebuilds the whole scene; here the caller redraws the flagged
@@ -41,6 +43,9 @@ MAX_OBJECTS = 64
 MODIFY = {"stack": 1, "lift": 2, "train": 3, "reach": 4}
 # goals/pickandplace.py:15, goals/object_state.py GoalArgs.height_range
 HEIGHT_RANGE = (0.05, 0.25)
+LAYOUT = {"domino": 1, "attached": 2, "fixed": 3}
+DOMINO_MAX_RETRY = 1000         # goals/dominos.py MAX_RETRY
+ATTACHED_BLOCKS = 8             # goals/attached_block_state.py: the pattern's cells
 
 
 def table_dimensions(model):
@@ -271,6 +276,123 @@ def reach_goals(bbox, active, table, area, seed, epoch, target_height, mask=None
     pos, status = _place(bbox, act, table, area, seed, epoch, "uniform", mask, out, max_trials, max_per_object, None, 1.0, GOAL_DISTANCE_MIN)
     obj = pos.clone()
     return _modify("reach", pos, act, seed, epoch, mask, target_height=target_height), obj, status
+
+
+def _layout(kind, bbox, active, table, area, seed, epoch, mask, out, object_size=None, distance_mul=None, rel=None, max_retry=1):
+    """rg_layout_goals: (pos, quat, status, angle, retry); angle and retry only for dominoes (else None)"""
+    import torch as t
+
+    nenv, nobj, dev = _bbox_shape(bbox)
+    if tuple(bbox.shape[2:]) != (2, 3):
+        raise ValueError("bbox: [nenv, nobj, 2, 3] (center, half size)")
+    if nobj > MAX_OBJECTS:
+        raise ValueError(f"at most {MAX_OBJECTS} objects per environment")
+    bb = bbox.to(t.float64).contiguous()
+    if not bool(t.isfinite(bb).all()) or bool((bb[:, :, 1] < 0).any()):
+        raise ValueError("bbox: finite, with half sizes >= 0")
+    if not (0 <= int(seed) < 1 << 32 and 0 <= int(epoch) < 1 << 32):
+        raise ValueError("seed and epoch: 32-bit unsigned integers")
+    act, n = _active_counts(t, active, mask, nenv, nobj, dev)
+    ar = as_device(t, area, t.float64, (nenv, 6), "area", dev)
+    tab = np.concatenate([np.asarray(table[0], dtype=np.float64).reshape(3), np.asarray(table[1], dtype=np.float64).reshape(3)])
+    per = {}
+    for name, v in (("object_size", object_size), ("distance_mul", distance_mul)):
+        if v is not None:
+            per[name] = as_device(t, v, t.float64, (nenv,), name, dev)
+            if not bool((t.isfinite(per[name]) & (per[name] > 0)).all()):
+                raise ValueError(f"{name}: finite and > 0")
+    if out is None:
+        pos = t.zeros(nenv, nobj, 3, dtype=t.float64, device=dev)
+        quat = t.zeros(nenv, nobj, 4, dtype=t.float64, device=dev)
+        quat[..., 0] = 1.0
+    else:
+        pos, quat = out
+        for name, x, w in (("pos", pos, 3), ("quat", quat, 4)):
+            if not t.is_tensor(x) or x.dtype != t.float64 or tuple(x.shape) != (nenv, nobj, w) or not x.is_contiguous() or x.device != dev:
+                raise ValueError(f"out: (pos, quat), contiguous float64 tensors [nenv, nobj, 3] and [nenv, nobj, 4] on the device of bbox ({name})")
+    status = t.full((nenv,), -1, dtype=t.int32, device=dev)
+    angle = retry = None
+    if kind == "domino":
+        angle = t.zeros(nenv, nobj, dtype=t.float64, device=dev)
+        retry = t.full((nenv,), -1, dtype=t.int32, device=dev)
+    mk = device_mask(t, mask, nenv, dev)
+    with t.cuda.device(dev):
+        engine._check(engine.lib().rg_layout_goals(nenv, nobj, LAYOUT[kind], ptr(bb), ptr(act), tab.ctypes.data, ptr(ar), ptr(per.get("object_size")),
+                                                   ptr(per.get("distance_mul")), ptr(rel), int(max_retry), int(seed), int(epoch), ptr(mk), ptr(pos),
+                                                   ptr(quat), ptr(status), ptr(angle), ptr(retry), current_stream(t, dev)))
+    return pos, quat, status, angle, retry
+
+
+def domino_goals(bbox, active, table, area, seed, epoch, object_size, distance_mul, max_retry=DOMINO_MAX_RETRY, mask=None, out=None, details=False):
+    """`DominoStateGoal._sample_next_goal_positions` (goals/dominos.py): the dominoes on a circle arc.  Each of up to max_retry
+    tries draws the arc's offset and step, turns domino i by i * step + (offset + step / 2) about z, lays the dominoes
+    object_size * distance_mul apart along the arc and keeps the first arc whose turned boxes fit in the placement area, moved
+    to a uniform spot in it.  bbox: the unrotated boxes ([nenv, nobj, 2, 3] CUDA, bounding_boxes with the identity);
+    object_size and distance_mul (domino_distance_mul): [nenv] or scalars, > 0.  Every selected environment needs an active
+    object.  Returns (pos [nenv, nobj, 3], quat [nenv, nobj, 4] the z rotations, status [nenv] int32: 1 placed, 0 no arc fitted
+    within max_retry -- positions zeroed, as the reference returns with goal_valid False --, -1 not selected by `mask`).
+    `out` = (pos, quat) is written in place on the selected environments' active slots.  details=True adds angle [nenv, nobj]
+    (the z angles) and retry [nenv] (the arc that fitted, -1 none).  Evaluate with rot_dist_type="mod180", as the reference's
+    dominos environment does."""
+    import torch as t
+
+    if int(max_retry) < 1:
+        raise ValueError("max_retry must be >= 1")
+    nenv, nobj, dev = _bbox_shape(bbox)
+    _, n = _active_counts(t, active, mask, nenv, nobj, dev)
+    if (n == 0).any():
+        raise ValueError("domino_goals: every selected environment needs an active object")
+    pos, quat, status, angle, retry = _layout("domino", bbox, active, table, area, seed, epoch, mask, out, object_size=object_size,
+                                              distance_mul=distance_mul, max_retry=max_retry)
+    return (pos, quat, status, angle, retry) if details else (pos, quat, status)
+
+
+def attached_goals(bbox, active, table, area, seed, epoch, object_size, mask=None, out=None):
+    """`AttachedBlockStateGoal._sample_next_goal_positions` (goals/attached_block_state.py): eight blocks tightly attached in
+    the reference's pattern (two rows of two around a row of four, cells of object_size * 2 in placement-area units), the rows
+    permuted among the blocks and the pattern moved to a uniform origin in the area, then place_targets_with_fixed_position.
+    object_size: [nenv] or a scalar, > 0.  Every selected environment needs exactly 8 active blocks, as the reference's
+    blocks_attached environment has.  Returns (pos, quat, status) as domino_goals, with identity rotations and status 1."""
+    import torch as t
+
+    nenv, nobj, dev = _bbox_shape(bbox)
+    _, n = _active_counts(t, active, mask, nenv, nobj, dev)
+    if ((n >= 0) & (n != ATTACHED_BLOCKS)).any():
+        raise ValueError(f"attached_goals: every selected environment needs exactly {ATTACHED_BLOCKS} active blocks")
+    return _layout("attached", bbox, active, table, area, seed, epoch, mask, out, object_size=object_size)[:3]
+
+
+def fixed_goals(bbox, active, table, area, relative_placements, init_quat=None, mask=None, out=None):
+    """`ObjectFixedStateGoal._sample_next_goal_positions` (goals/object_state_fixed.py, the table_setting and wordblocks
+    goals): place_targets_with_fixed_position of relative_placements ([nenv, nobj, 2] or [nobj, 2], each object's (x, y) as a
+    fraction of the placement area; values outside [0, 1] are used as they are, as the reference does).  init_quat ([nenv,
+    nobj, 4] or [nobj, 4], w x y z; None = identity) becomes the goal rotation with w >= 0 (set_target_quat's
+    quat_normalize).  No random numbers.  Returns (pos, quat, status) as domino_goals, status 1."""
+    import torch as t
+
+    nenv, nobj, dev = _bbox_shape(bbox)
+    rp = t.as_tensor(relative_placements.cpu() if t.is_tensor(relative_placements) else np.asarray(relative_placements, dtype=np.float64))
+    if tuple(rp.shape) not in ((nobj, 2), (nenv, nobj, 2)):
+        raise ValueError("relative_placements: [nobj, 2] or [nenv, nobj, 2]")
+    rel = rp.to(device=dev, dtype=t.float64).expand(nenv, nobj, 2).contiguous()
+    if not bool(t.isfinite(rel).all()):
+        raise ValueError("relative_placements: finite")
+    q0 = None
+    if init_quat is not None:
+        iq = t.as_tensor(init_quat.cpu() if t.is_tensor(init_quat) else np.asarray(init_quat, dtype=np.float64))
+        if tuple(iq.shape) not in ((nobj, 4), (nenv, nobj, 4)):
+            raise ValueError("init_quat: [nobj, 4] or [nenv, nobj, 4]")
+        q0 = iq.to(device=dev, dtype=t.float64).expand(nenv, nobj, 4)
+        if not bool(t.isfinite(q0).all()) or bool((q0.norm(dim=2) == 0).any()):
+            raise ValueError("init_quat: finite and non-zero")
+        q0 = t.where(q0[..., :1] < 0, -q0, q0)
+    pos, quat, status = _layout("fixed", bbox, active, table, area, 0, 0, mask, out, rel=rel)[:3]
+    if q0 is not None:
+        act = as_device(t, active, t.bool, (nenv, nobj), "active", dev)
+        if mask is not None:
+            act = act & as_device(t, mask, t.bool, (nenv,), "mask", dev)[:, None]
+        quat.copy_(t.where(act[..., None], q0, quat))
+    return pos, quat, status
 
 
 def body_aabb(sim, bodies, quat=None, mask=None):
