@@ -163,6 +163,11 @@ int rg_model_origin(const rg_model* m, float origin[3]);
 int rg_batch_set_balance(rg_batch* b, int on);
 /* launch geometry actually used (for reporting): CTAs, warps per CTA, dynamic shared bytes */
 int rg_batch_launch_info(const rg_batch* b, int* ctas, int* warps_per_cta, int* smem_bytes);
+/* warps that step one environment: 1 = one warp per environment (warps_per_cta environments per CTA), 2..16 = one environment per
+ * CTA of that many warps, which share the dense part of its constraint solve with bit-identical results.  Chosen at batch
+ * creation for models whose scratch leaves a single environment per SM and whose solver is large; the environment variable
+ * RG_WARPS_PER_ENV=1|2|4|8|16 forces it. */
+int rg_batch_env_warps(const rg_batch* b, int* warps_per_env);
 
 /* nsub x mj_step, then `final_forward` x mj_forward (0..4: SimulationInterface.step ends with one sim.forward(); the
  * observation path of RobotEnv runs more of them (robogym/robot_env.py:677, observation/mujoco.py:27) and mujoco-py's

@@ -6,15 +6,19 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "librobogym_b200.so")
-DEPS = [os.path.join(SRC, f) for f in ("rg_engine.cu", "rg_defs.h", "rg_dyn.inl", "rg_col.inl", "rg_sol.inl", "rg_step.inl", "rg_place.inl", "rg_goal.inl", "rg_obs.inl", "rg_host.h", "rg_derived_fields.h")]
+DEPS = [os.path.join(SRC, f) for f in ("rg_engine.cu", "rg_cta.cu", "rg_kernel.inl", "rg_defs.h", "rg_dyn.inl", "rg_col.inl", "rg_sol.inl", "rg_step.inl", "rg_place.inl", "rg_goal.inl", "rg_obs.inl", "rg_host.h", "rg_derived_fields.h")]
 DEPS += [os.path.join(HERE, "..", "include", f) for f in ("rg_model_fields.h", "robogym_b200.h")]
 
 
-def nvcc_cmd(extra=()):
+# the one-warp kernel (rg_engine.cu, with the C ABI) and the one-environment-per-CTA kernel (rg_cta.cu), linked into one library
+SOURCES = ("rg_engine.cu", "rg_cta.cu")
+
+
+def nvcc_cmd(extra=(), sources=("rg_engine.cu",)):
     nvcc = os.environ.get("NVCC", "nvcc")
     # -prec-div/-prec-sqrt=false: 2-ulp division / square root without the slow-path calls (measured +6 %, parity unchanged)
     return [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-prec-div=false", "-prec-sqrt=false", "-ftz=true",
-            "-Xcompiler", "-fPIC", "-shared", *extra, "-o", OUT, os.path.join(SRC, "rg_engine.cu")]
+            "-Xcompiler", "-fPIC", "-shared", *extra, "-o", OUT, *[os.path.join(SRC, s) for s in sources]]
 
 
 def _fresh():
@@ -31,7 +35,7 @@ def build(force=False, verbose=False):
         fcntl.flock(lock, fcntl.LOCK_EX)
         try:
             if force or not _fresh():
-                cmd = nvcc_cmd(("-Xptxas", "-v") if verbose else ())
+                cmd = nvcc_cmd(("-Xptxas", "-v") if verbose else (), SOURCES)
                 tmp = OUT + ".tmp.%d" % os.getpid()
                 cmd[cmd.index("-o") + 1] = tmp
                 subprocess.check_call(cmd)
@@ -45,7 +49,7 @@ def build_profile(level=1):
     """Same engine with per-stage clock64 counters in the RG_DBG dump (profiling only); level 2 breaks the Newton solve
     down instead of the collision stage."""
     out = os.path.join(HERE, "librobogym_b200_prof%s.so" % ("" if level == 1 else str(level)))
-    cmd = nvcc_cmd(("-DRG_PROFILE=%d" % level,))
+    cmd = nvcc_cmd(("-DRG_PROFILE=%d" % level,), SOURCES)
     cmd[cmd.index("-o") + 1] = out
     subprocess.check_call(cmd)
     return out
@@ -57,7 +61,7 @@ def build_variant(tag, defines):
     flags = []
     for d in defines:                      # "-..." entries are raw nvcc flags ("+" stands for a space), the rest are -D macros
         flags += d.split() if d.startswith("-") else ["-D" + d]
-    cmd = nvcc_cmd(tuple(flags))
+    cmd = nvcc_cmd(tuple(flags), SOURCES)
     cmd[cmd.index("-o") + 1] = out
     subprocess.check_call(cmd)
     return out

@@ -42,7 +42,11 @@
 #include <cuda_runtime.h>
 #include <string.h>
 #define RG_DEV __device__ __forceinline__
+#ifdef RG_COOP   /* internal linkage: rg_cta.cu compiles the same functions again, into the same library as rg_engine.cu */
+#define RG_DEV_NOINLINE static __device__ __noinline__
+#else
 #define RG_DEV_NOINLINE __device__ __noinline__
+#endif
 /* lane-strided loops run once or twice (n <= 64): unrolling them only bloats a kernel that is instruction-cache bound */
 #define RG_NOUNROLL _Pragma("unroll 1")
 #define RG_UNROLL2 _Pragma("unroll 2")
@@ -108,6 +112,56 @@ __device__ __forceinline__ void rg_stage_sync() {
 #endif
 #define RG_CTA_ANY(x) __syncthreads_or(x)
 #define RG_SINCOS(x, sn, cs) __sincosf(x, sn, cs)
+#endif
+
+/* Cooperative sections.  -DRG_COOP builds (rg_cta.cu, tests/emu/rg_emu_cta.cpp) run ONE environment per CTA of W warps: warp 0
+ * runs every stage as above, and the dense per-element loops of the Newton solve (rg_sol.inl: the Hessian assembly, the
+ * envelope Cholesky, the triangular solves, the matrix-vector products) spread their outputs over all RG_NT = 32 W threads.
+ * Each output element is still computed by one thread with the same operation sequence, so the results are the one-warp
+ * results bit for bit; only the owner of an element changes.  A cooperative phase ends at named barrier RG_COOP_BAR over the
+ * CTA (the stage barriers use 0 and 1..RG_BAR_GROUPS).  A value one thread hands to all (RG_COOP_PUT / RG_COOP_BCAST) goes
+ * through shared memory instead of a shuffle.  Without RG_COOP every macro below is the one-warp phase it stands for. */
+#ifndef RG_COOP
+#define RG_NT 32
+#define RG_COOP_LANE_DECL RG_LANE_DECL
+#define RG_COOP_BEGIN RG_PHASE_BEGIN
+#define RG_COOP_END RG_PHASE_END
+#define COOPVAR(T, x) LANEVAR(T, x)
+#define COOPARR(T, x, n) LANEARR(T, x, n)
+#define RG_COOP_PUT(k, who, v)
+#define RG_COOP_BCAST(x, k, src) RG_WARP_BCAST(x, src)
+#define RG_COOP_ENTER(id, c, a0, a1, a2, a3, a4, a5, p)
+#elif defined(RG_EMU)
+extern int rg_emu_coop_threads;   /* 32 W of the emulated CTA */
+#define RG_NT rg_emu_coop_threads
+#define RG_COOP_LANE_DECL
+#define RG_COOP_BEGIN for (int lane = 0; lane < RG_NT; ++lane) {
+#define RG_COOP_END }
+#define COOPVAR(T, x) T x[512]
+#define COOPARR(T, x, n) T x[512][n]
+#define RG_COOP_PUT(k, who, v)
+#define RG_COOP_BCAST(x, k, src) (x[src])
+#define RG_COOP_ENTER(id, c, a0, a1, a2, a3, a4, a5, p)
+#else
+#define RG_COOP_BAR 15
+#define RG_NT ((int)blockDim.x)
+__shared__ float rg_coop_bc[2];   /* RG_COOP_PUT slots */
+RG_DEV void rg_coop_sync() { asm volatile("bar.sync %0, %1;" ::"r"(RG_COOP_BAR), "r"((int)blockDim.x) : "memory"); }
+#define RG_COOP_LANE_DECL const int lane = threadIdx.x;
+#define RG_COOP_BEGIN {
+#define RG_COOP_END } rg_coop_sync();
+#define COOPVAR(T, x) T x
+#define COOPARR(T, x, n) T x[n]
+#define RG_COOP_PUT(k, who, v) if (who) rg_coop_bc[k] = (float)(v);
+#define RG_COOP_BCAST(x, k, src) rg_coop_bc[k]
+/* warp 0 enters a cooperative section: it posts the section and its arguments, and the other warps, waiting in rg_coop_worker
+   (rg_sol.inl), join it */
+#define RG_COOP_ENTER(id, c, a0, a1, a2, a3, a4, a5, p) if (threadIdx.x < 32) rg_coop_post(id, c, a0, a1, a2, a3, a4, a5, p);
+/* one environment per CTA: warp 0 runs the stages alone, so the stage barriers have nobody to wait for */
+#undef RG_CTA_SYNC
+#undef RG_CTA_ANY
+#define RG_CTA_SYNC() __syncwarp()
+#define RG_CTA_ANY(x) (x)
 #endif
 
 #define RG_MINVAL 1e-15f

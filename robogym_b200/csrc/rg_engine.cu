@@ -35,121 +35,31 @@
 #ifndef RG_NARROW_WARPS
 #define RG_NARROW_WARPS 12
 #endif
+/* One environment per CTA of RG_CTA_WARPS warps (rg_cta.cu) for the models whose one-warp scratch leaves a single environment
+   per SM and whose constraint solver has at least RG_CTA_MIN_NS dofs: there the dense solve is the part the other warps of the
+   SM can take (DESIGN.md section 8, cfg 3).  RG_WARPS_PER_ENV=1|2|4|8|16 overrides the choice for any model. */
+#ifndef RG_CTA_WARPS
+#define RG_CTA_WARPS 8
+#endif
+#ifndef RG_CTA_MIN_NS
+#define RG_CTA_MIN_NS 96
+#endif
 
 static thread_local std::string g_err;
 static int rg_fail(int code, const std::string& msg) { g_err = msg; return code; }
 #define RG_CUDA(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) return rg_fail(-2, std::string(#call) + ": " + cudaGetErrorString(e_)); } while (0)
 
-struct RgKernelArgs {
-  RgModel m;          /* host-style view whose pointers point into the DEVICE arena (source of the staged copy) */
-  RgLayout L;
-  RgBatchIO io;
-  const char* arena;  /* device arena base (16B aligned) */
-  int nsub, final_forward, warps;
-  int groups;              /* barrier groups per round (>= 1) */
-  /* per-environment overrides of float model arrays (domain randomisation) */
-  int nover;
-  int over_floats;                               /* floats of the per-warp override area */
-  int over_off[RG_MAX_PARAM_OVERRIDES];          /* byte offset of the RgArr member inside RgModelDev */
-  int over_cnt[RG_MAX_PARAM_OVERRIDES];          /* floats per environment */
-  int over_dst[RG_MAX_PARAM_OVERRIDES];          /* float offset inside the per-warp override area */
-  const float* over_ptr[RG_MAX_PARAM_OVERRIDES]; /* [nenv][cnt] in global memory */
-  const int* order;   /* [nenv] slot -> environment (work-sorted, see rg_order_kernel) or nullptr = identity */
-  const int* nslots;  /* device: number of slots of a subset launch (rg_step_subset) or nullptr = every environment */
-  int* counter;       /* device: next unassigned slot of this launch (zeroed before the launch) */
-  int setconst[6];    /* nsub < 0 = an rg_set_const launch: override slots of dof_invweight0, body_invweight0, tendon_invweight0,
-                         tendon_length0, body_subtreemass, opt_meaninertia (-1 = not bound per environment, not written) */
-  /* per-environment pair lists (rg_batch_update_pairs) or nullptr = every environment streams the static list */
-  const unsigned* env_pairs;   /* [nenv][pair_cap] g1 | g2 << 16 */
-  const int* env_npair;        /* [nenv] */
-  int pair_cap;
-};
-
-__device__ __forceinline__ uint32_t rg_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-#define RG_MODEL_DEV_BYTES ((int)((sizeof(RgModelDev) + 127) & ~(size_t)127))
-/* every warp with overrides keeps its own copy of the view: 128 B more would cost dactyl/locked a resident environment per SM */
-static_assert(sizeof(RgModelDev) <= 1024, "the device model view must fit in 1024 bytes of shared memory");
+#include "rg_kernel.inl"
 
 template <int MAXW>
 __global__ void __launch_bounds__(MAXW * 32, 1) rg_step_kernel(const __grid_constant__ RgKernelArgs args) {
-  unsigned char* smem_raw = rg_smem_raw;
   __shared__ __align__(8) unsigned long long mbar;
-  /* dynamic shared layout: [RgModelDev] [small model arena] [warps x scratch] [warps x (RgModelDev + override rows)] */
-  RgModelDev* sm = (RgModelDev*)smem_raw;
+  float* scratch0 = rg_kernel_stage(args, &mbar);
   const int model_bytes = RG_MODEL_DEV_BYTES;
-  unsigned char* sarena = smem_raw + model_bytes;
-  const int small_bytes = args.m.small_bytes;
-  float* scratch0 = (float*)(sarena + ((small_bytes + 127) & ~127));
-
-  /* ---- stage the small model arrays with one TMA bulk copy */
-  if (threadIdx.x == 0) {
-    const uint32_t bar = rg_smem_u32(&mbar);
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
-#if RG_SKEW > 0
-    for (int i = 0; i < RG_BAR_RING; i++) asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(rg_smem_u32(&rg_stage_bar[i])), "r"((uint32_t)args.warps));
-    for (int i = 0; i < 32; i++) rg_stage_k[i] = 0;
-#endif
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)small_bytes) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(rg_smem_u32(sarena)), "l"(args.arena), "r"((uint32_t)small_bytes), "r"(bar) : "memory");
-  }
-  /* meanwhile: the device model view (shared-memory offsets of the staged arrays, global pointers of the big ones) */
-  if (threadIdx.x < 32) {
-    const int lane = threadIdx.x;
-    int k = 0;
-    const char* abase = args.arena;
-#define RG_SETOFF(field) { if (lane == (k & 31)) sm->field.off = model_bytes + (int)((const char*)args.m.field - abase); k++; }
-#define RG_SETPTR(field) { if (lane == (k & 31)) sm->field = args.m.field; k++; }
-#define RG_DIM(n) { if (lane == (k & 31)) sm->n = args.m.n; k++; }
-#define RG_I(n, c) RG_SETOFF(n)
-#define RG_F(n, c) RG_SETOFF(n)
-#define RG_IB(n, c) RG_SETPTR(n)
-#define RG_FB(n, c) RG_SETPTR(n)
-#include "../../include/rg_model_fields.h"
-#undef RG_DIM
-#undef RG_I
-#undef RG_F
-#undef RG_IB
-#undef RG_FB
-#define RG_DS(n, T, c) RG_SETOFF(n)
-#define RG_DG(n, T, c) RG_SETPTR(n)
-#define RG_DGH(n, T, c)
-#include "rg_derived_fields.h"
-    if (lane == 0) {
-      sm->has_pairs = args.m.pair_packed != nullptr;
-      /* per-environment arrays are unbound: every factor 1 (a bound row overwrites the offset in the warp's own view) */
-#define RG_DE(n, T, c) sm->n.off = -1;
-#include "rg_derived_fields.h"
-#define RG_DSO(n, T, c, when) sm->n.off = args.m.n ? model_bytes + (int)((const char*)args.m.n - abase) : 0;
-#include "rg_derived_fields.h"
-      sm->origin[0] = args.m.origin[0]; sm->origin[1] = args.m.origin[1]; sm->origin[2] = args.m.origin[2];
-      sm->small_bytes = small_bytes;
-      sm->nM = args.m.nM;
-      sm->ndoflevel = args.m.ndoflevel;
-      sm->ns = args.m.ns;
-      sm->neqrow = args.m.neqrow;
-      sm->pidw = args.m.pidw;
-    }
-    for (int i = lane; i < (int)(sizeof(RgLayout) / 4); i += 32) ((int*)&sm->L)[i] = ((const int*)&args.L)[i];
-#undef RG_SETOFF
-#undef RG_SETPTR
-  }
-  __syncthreads();
-  {
-    const uint32_t bar = rg_smem_u32(&mbar);
-    uint32_t done = 0;
-    while (!done) {
-      asm volatile("{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n selp.u32 %0, 1, 0, p;\n}" : "=r"(done) : "r"(bar), "r"(0u) : "memory");
-    }
-  }
-  __syncthreads();
-
   const int warp = threadIdx.x >> 5;
   float* s = scratch0 + (size_t)warp * args.L.total;   /* L.total is a multiple of 4 floats: every per-warp area stays 16-byte aligned */
   /* with per-env overrides every warp keeps its own model view + a copy of this env's rows after the scratch */
-  RgModelDev* wm = sm;
+  RgModelDev* wm = (RgModelDev*)rg_smem_raw;
   float* wover = nullptr;
   if (args.nover > 0 || args.env_pairs) {
     unsigned char* base = (unsigned char*)(scratch0 + (size_t)args.warps * args.L.total) + (size_t)warp * (model_bytes + 4 * args.over_floats);
@@ -177,32 +87,8 @@ __global__ void __launch_bounds__(MAXW * 32, 1) rg_step_kernel(const __grid_cons
     __syncthreads();
     if (warp >= nact) continue;
     const int e = args.order ? args.order[slot0 + warp] : slot0 + warp;
-    if (args.nover > 0 || args.env_pairs) {
-      const int lane = threadIdx.x & 31;
-      for (int i = lane; i < (int)(sizeof(RgModelDev) / 4); i += 32) ((int*)wm)[i] = ((const int*)sm)[i];
-      /* plain 32-bit loads and stores: the int rows of geom_dataid pass through this float copy bit for bit */
-      for (int o = 0; o < args.nover; o++) {
-        const float* src = args.over_ptr[o] + (size_t)e * args.over_cnt[o];
-        for (int i = lane; i < args.over_cnt[o]; i += 32) wover[args.over_dst[o] + i] = src[i];
-      }
-      __syncwarp();
-      if (lane < args.nover) *(int*)((char*)wm + args.over_off[lane]) = (int)((unsigned char*)(wover + args.over_dst[lane]) - rg_smem_raw);
-      if (args.env_pairs && lane == 0) {   /* stage A streams this environment's own list (rg_pair) */
-        wm->has_pairs = 0;
-        wm->pair_geom1 = (const int*)(args.env_pairs + (size_t)e * args.pair_cap);
-        wm->pair_geom2 = nullptr;
-        wm->npair = args.env_npair[e];
-      }
-      __syncwarp();
-    }
-    if (args.nsub < 0) {
-      RgSetConstOut o;
-      float** op = (float**)&o;
-      for (int k = 0; k < 6; k++) op[k] = args.setconst[k] >= 0 ? (float*)args.over_ptr[args.setconst[k]] + (size_t)e * args.over_cnt[args.setconst[k]] : nullptr;
-      rg_env_setconst((int)((unsigned char*)wm - rg_smem_raw), args.L, s, (int)(s - (float*)rg_smem_raw), o);
-      continue;
-    }
-    rg_env_step((int)((unsigned char*)wm - rg_smem_raw), args.L, s, (int)(s - (float*)rg_smem_raw), args.io, e, args.nsub, args.final_forward, 1);
+    if (args.nover > 0 || args.env_pairs) rg_kernel_env_view(args, wm, wover, e);
+    rg_kernel_env(args, wm, s, e);
   }
 }
 
@@ -375,6 +261,7 @@ struct rg_batch {
   int nenv;
   void* ptr[RG_NFIELDS];
   int ctas, warps, smem;
+  int env_warps = 1;       /* warps per environment: 1 = rg_step_kernel, 2..16 = rg_step_cta_kernel (one environment per CTA) */
   int nover = 0;
   int over_off[RG_MAX_PARAM_OVERRIDES], over_cnt[RG_MAX_PARAM_OVERRIDES], over_dst[RG_MAX_PARAM_OVERRIDES];
   int over_floats = 0;
@@ -586,6 +473,22 @@ static int rg_batch_size(rg_batch* b) {
   const int per_warp = 4 * b->L.total + (b->nover > 0 || b->d_pairs ? model_bytes + 4 * b->over_floats : 0);
   int warps = (maxsmem - fixed) / per_warp;
   if (warps < 1) return rg_fail(-3, "rg_batch: model scratch does not fit in shared memory");
+  int env_warps = warps == 1 && m->hm.view.ns >= RG_CTA_MIN_NS ? RG_CTA_WARPS : 1;
+  const char* eenv = getenv("RG_WARPS_PER_ENV");
+  if (eenv) {
+    const int w = atoi(eenv);
+    if (w == 1 || w == 2 || w == 4 || w == 8 || w == 16) env_warps = w;
+  }
+  b->env_warps = env_warps;
+  if (env_warps > 1) {
+    int cta_static = 0;
+    RG_CUDA(rg_cta_prepare(env_warps, maxsmem + (int)fa.sharedSizeBytes, &cta_static));   /* (the opt-in limit, less its own static shared memory) */
+    if (per_warp + fixed > maxsmem + (int)fa.sharedSizeBytes - cta_static) return rg_fail(-3, "rg_batch: model scratch does not fit in shared memory");
+    b->warps = 1;   /* environments per CTA */
+    b->smem = fixed - 64 + per_warp;
+    b->ctas = nenv < sms ? nenv : sms;
+    return 0;
+  }
   if (warps > RG_MAX_WARPS) warps = RG_MAX_WARPS;
   /* rounds are handed out dynamically and a partial round runs with fewer warps, so more resident warps never cost padding */
   if (warps > nenv) warps = nenv;
@@ -809,6 +712,12 @@ int rg_batch_launch_info(const rg_batch* b, int* ctas, int* warps, int* smem) {
   return 0;
 }
 
+int rg_batch_env_warps(const rg_batch* b, int* warps_per_env) {
+  if (!b || !warps_per_env) return rg_fail(-1, "rg_batch_env_warps: null argument");
+  *warps_per_env = b->env_warps;
+  return 0;
+}
+
 static int rg_fill_io(const rg_batch* b, RgBatchIO& io) {
   for (int f = RG_FIELD_QPOS; f <= RG_FIELD_WARMSTART; f++)
     if (!b->ptr[f] && !((f == RG_FIELD_CTRL || f == RG_FIELD_PID) && b->model->hm.view.nu == 0))   /* a model without actuators has no ctrl / PID rows */
@@ -870,7 +779,8 @@ static int rg_launch_step(rg_batch* b, const uint8_t* mask, int nsub, int final_
   }
   args.counter = b->d_counter;
   RG_CUDA(cudaMemsetAsync(b->d_counter, 0, sizeof(int), (cudaStream_t)stream));
-  if (b->warps > RG_NARROW_WARPS) rg_step_kernel<RG_MAX_WARPS><<<b->ctas, 32 * b->warps, b->smem, (cudaStream_t)stream>>>(args);
+  if (b->env_warps > 1) RG_CUDA(rg_cta_launch(b->env_warps, b->ctas, b->smem, (cudaStream_t)stream, args));
+  else if (b->warps > RG_NARROW_WARPS) rg_step_kernel<RG_MAX_WARPS><<<b->ctas, 32 * b->warps, b->smem, (cudaStream_t)stream>>>(args);
   else rg_step_kernel<RG_NARROW_WARPS><<<b->ctas, 32 * b->warps, b->smem, (cudaStream_t)stream>>>(args);
   RG_CUDA(cudaGetLastError());
   if (!mask && b->balance && nsub > 0) {   /* (not after rg_set_const: it leaves no cost) */

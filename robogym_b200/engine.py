@@ -91,6 +91,7 @@ SIGNATURES = {
     "rg_model_origin": (_ci, [_vp, _P(ctypes.c_float)]),
     "rg_batch_set_balance": (_ci, [_vp, _ci]),
     "rg_batch_launch_info": (_ci, [_vp, _P(_ci), _P(_ci), _P(_ci)]),
+    "rg_batch_env_warps": (_ci, [_vp, _P(_ci)]),
     "rg_step": (_ci, [_vp, _ci, _ci, _vp]),
     "rg_forward": (_ci, [_vp, _vp]),
     "rg_step_subset": (_ci, [_vp, _vp, _ci, _ci, _vp]),
@@ -454,9 +455,10 @@ class BatchedSim:
         _check(lib().rg_batch_set_balance(self.h, int(bool(on))))
 
     def launch_info(self):
-        a, b, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
+        a, b, c, w = ctypes.c_int(), ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
         lib().rg_batch_launch_info(self.h, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c))
-        return dict(ctas=a.value, warps_per_cta=b.value, smem_bytes=c.value, scratch_bytes_per_env=lib().rg_batch_scratch_bytes(self.h),
+        _check(lib().rg_batch_env_warps(self.h, ctypes.byref(w)))
+        return dict(ctas=a.value, warps_per_cta=b.value, warps_per_env=w.value, smem_bytes=c.value, scratch_bytes_per_env=lib().rg_batch_scratch_bytes(self.h),
                     contact_capacity=self.contact_capacity, row_capacity=self.row_capacity, dofs_per_contact=self.dofs_per_contact)
 
     def dbg_view(self, env=0):
