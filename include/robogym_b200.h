@@ -178,6 +178,16 @@ int rg_forward(rg_batch* b, void* stream);
  * nothing (the launch covers only the selected environments).  What a Python loop over MjSim objects does when it
  * calls sim.forward()/sim.step() on some environments only (goal switches, resets). */
 int rg_step_subset(rg_batch* b, const uint8_t* mask_device, int nsub, int final_forward, void* stream);
+/* The reference's stabilize_objects (robogym/envs/rearrange/common/utils.py:76-93) for the environments whose mask byte is
+ * non-zero (mask == NULL: all): nsub x mj_step with dof_damping[d] = `damping` for each of the `ndof` dof ids in the HOST array
+ * `dofs` (1..64 ids in [0, nv); the same value for every selected environment, float32 on the device), then `final_forward` x
+ * mj_forward (0..4) with each environment's own damping, as the reference's forward() after restoring it.  Neither the model
+ * nor a per-environment dof_damping row changes.  The result is byte-identical to binding dof_damping per environment with
+ * those entries set in the selected environments, rg_step_subset(mask, nsub, 0), restoring the rows and
+ * rg_step_subset(mask, 0, final_forward); without the per-environment rows, which a batch would otherwise carry on every step.
+ * Refused: an empty or out-of-range dof list, a negative or non-finite damping, and batches with rg_batch_env_warps > 1.
+ * Two launches, asynchronous on `stream`. */
+int rg_step_settle(rg_batch* b, const uint8_t* mask_device, const int* dofs, int ndof, double damping, int nsub, int final_forward, void* stream);
 /* mj_setConst per environment (SimulationInterface.set_constants, robogym/mujoco/simulation_interface.py:197-201, which the
  * reference calls after its randomisers edited masses, inertias, armatures ...): recomputes, from each selected environment's
  * own parameter view at qpos0, the constants MuJoCo derives from the model -- dof_invweight0, body_invweight0,

@@ -324,6 +324,15 @@ typedef const RgModel* RgMRef;
 #define RG_MDEREF(r) (*(r))
 #define RG_MREF(m) (&(m))
 #endif
+/* the two reads of dof_damping: the passive force (rg_forces) and the implicit term of the Euler factor (rg_euler).  Both go
+   through the model view, which is where the settle launch puts its override (rg_kernel.inl); the CPU emulation can redirect
+   one of them at a time to show that the override reaches both (tests/emu/rg_emu_settle.cpp). */
+#ifndef RG_DAMPING_PASSIVE
+#define RG_DAMPING_PASSIVE(m) (m).dof_damping
+#endif
+#ifndef RG_DAMPING_IMPLICIT
+#define RG_DAMPING_IMPLICIT(m) (m).dof_damping
+#endif
 
 
 #ifndef RG_EMU

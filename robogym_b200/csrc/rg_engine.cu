@@ -51,10 +51,16 @@ static int rg_fail(int code, const std::string& msg) { g_err = msg; return code;
 
 #include "rg_kernel.inl"
 
-template <int MAXW>
-__global__ void __launch_bounds__(MAXW * 32, 1) rg_step_kernel(const __grid_constant__ RgKernelArgs args) {
+/* The step kernel's body.  SETTLE = the settle launch (rg_step_settle): the listed dofs' damping is overridden in the CTA's
+   staged model and in each environment's own dof_damping row; every other line is the default kernel's. */
+template <int MAXW, bool SETTLE>
+__device__ __forceinline__ void rg_step_body(const RgKernelArgs& args, const RgSettleArgs* st) {
   __shared__ __align__(8) unsigned long long mbar;
   float* scratch0 = rg_kernel_stage(args, &mbar);
+  if constexpr (SETTLE) {
+    rg_settle_patch(*st, (float*)(rg_smem_raw + ((const RgModelDev*)rg_smem_raw)->dof_damping.off), threadIdx.x, blockDim.x);
+    __syncthreads();
+  }
   const int model_bytes = RG_MODEL_DEV_BYTES;
   const int warp = threadIdx.x >> 5;
   float* s = scratch0 + (size_t)warp * args.L.total;   /* L.total is a multiple of 4 floats: every per-warp area stays 16-byte aligned */
@@ -88,8 +94,21 @@ __global__ void __launch_bounds__(MAXW * 32, 1) rg_step_kernel(const __grid_cons
     if (warp >= nact) continue;
     const int e = args.order ? args.order[slot0 + warp] : slot0 + warp;
     if (args.nover > 0 || args.env_pairs) rg_kernel_env_view(args, wm, wover, e);
+    if constexpr (SETTLE) {
+      if (st->row >= 0) { rg_settle_patch(*st, wover + st->row, threadIdx.x & 31, 32); __syncwarp(); }
+    }
     rg_kernel_env(args, wm, s, e);
   }
+}
+
+template <int MAXW>
+__global__ void __launch_bounds__(MAXW * 32, 1) rg_step_kernel(const __grid_constant__ RgKernelArgs args) {
+  rg_step_body<MAXW, false>(args, nullptr);
+}
+/* the same kernel with the settle flag set (rg_step_settle) */
+template <int MAXW>
+__global__ void __launch_bounds__(MAXW * 32, 1) rg_settle_kernel(const __grid_constant__ RgKernelArgs args, const __grid_constant__ RgSettleArgs st) {
+  rg_step_body<MAXW, true>(args, &st);
 }
 
 __global__ void rg_reset_kernel(RgModel m, RgBatchIO io, const uint8_t* mask) {
@@ -513,6 +532,8 @@ static int rg_batch_size(rg_batch* b) {
      device maximum once rather than to this batch's size */
   RG_CUDA(cudaFuncSetAttribute(rg_step_kernel<RG_NARROW_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsmem));
   RG_CUDA(cudaFuncSetAttribute(rg_step_kernel<RG_MAX_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsmem));
+  RG_CUDA(cudaFuncSetAttribute(rg_settle_kernel<RG_NARROW_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsmem));
+  RG_CUDA(cudaFuncSetAttribute(rg_settle_kernel<RG_MAX_WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, maxsmem));
   return 0;
 }
 
@@ -737,7 +758,7 @@ static int rg_fill_io(const rg_batch* b, RgBatchIO& io) {
   return 0;
 }
 
-static int rg_launch_step(rg_batch* b, const uint8_t* mask, int nsub, int final_forward, void* stream, bool setconst = false) {
+static int rg_launch_step(rg_batch* b, const uint8_t* mask, int nsub, int final_forward, void* stream, bool setconst = false, const RgSettleArgs* settle = nullptr) {
   if (!b || nsub < 0 || final_forward < 0 || final_forward > 4) return rg_fail(-1, "rg_step: bad argument");
   RgKernelArgs args;
   if (setconst) {
@@ -779,7 +800,10 @@ static int rg_launch_step(rg_batch* b, const uint8_t* mask, int nsub, int final_
   }
   args.counter = b->d_counter;
   RG_CUDA(cudaMemsetAsync(b->d_counter, 0, sizeof(int), (cudaStream_t)stream));
-  if (b->env_warps > 1) RG_CUDA(rg_cta_launch(b->env_warps, b->ctas, b->smem, (cudaStream_t)stream, args));
+  if (settle) {
+    if (b->warps > RG_NARROW_WARPS) rg_settle_kernel<RG_MAX_WARPS><<<b->ctas, 32 * b->warps, b->smem, (cudaStream_t)stream>>>(args, *settle);
+    else rg_settle_kernel<RG_NARROW_WARPS><<<b->ctas, 32 * b->warps, b->smem, (cudaStream_t)stream>>>(args, *settle);
+  } else if (b->env_warps > 1) RG_CUDA(rg_cta_launch(b->env_warps, b->ctas, b->smem, (cudaStream_t)stream, args));
   else if (b->warps > RG_NARROW_WARPS) rg_step_kernel<RG_MAX_WARPS><<<b->ctas, 32 * b->warps, b->smem, (cudaStream_t)stream>>>(args);
   else rg_step_kernel<RG_NARROW_WARPS><<<b->ctas, 32 * b->warps, b->smem, (cudaStream_t)stream>>>(args);
   RG_CUDA(cudaGetLastError());
@@ -795,6 +819,27 @@ int rg_step_subset(rg_batch* b, const uint8_t* mask, int nsub, int final_forward
   return rg_launch_step(b, mask, nsub, final_forward, stream);
 }
 int rg_forward(rg_batch* b, void* stream) { return rg_step(b, 0, 1, stream); }
+int rg_step_settle(rg_batch* b, const uint8_t* mask, const int* dofs, int ndof, double damping, int nsub, int final_forward, void* stream) {
+  if (ndof < 1 || ndof > RG_SETTLE_MAXDOF || !dofs) return rg_fail(-1, "rg_step_settle: the dof list must hold 1 to " + std::to_string(RG_SETTLE_MAXDOF) + " dofs");
+  if (!(damping >= 0.0) || !isfinite((float)damping)) return rg_fail(-1, "rg_step_settle: damping must be finite (in float32) and >= 0");
+  if (nsub < 0 || final_forward < 0 || final_forward > 4) return rg_fail(-1, "rg_step_settle: nsub must be >= 0 and final_forward 0..4");
+  if (!b) return rg_fail(-1, "rg_step_settle: null batch");
+  if (b->env_warps > 1) return rg_fail(-1, "rg_step_settle: batches with one environment per CTA (rg_batch_env_warps > 1) have no settle kernel");
+  RgSettleArgs st;
+  st.ndof = ndof; st.damping = (float)damping; st.row = -1;
+  const int nv = b->model->hm.view.nv;
+  for (int i = 0; i < ndof; i++) {
+    if (dofs[i] < 0 || dofs[i] >= nv) return rg_fail(-1, "rg_step_settle: dof id " + std::to_string(dofs[i]) + " out of range [0, " + std::to_string(nv) + ")");
+    st.dofs[i] = dofs[i];
+  }
+  const int slot = rg_find_override(b, "dof_damping");
+  if (slot >= 0) st.row = b->over_dst[slot];
+  /* the substeps with the override, then the final forward passes with the model's (or the environment's) own damping, as
+     the reference's forward() after restoring it: a launch of the default kernel */
+  int rc = rg_launch_step(b, mask, nsub, 0, stream, false, &st);
+  if (!rc && final_forward > 0) rc = rg_launch_step(b, mask, 0, final_forward, stream);
+  return rc;
+}
 int rg_set_const(rg_batch* b, const uint8_t* mask, void* stream) { return rg_launch_step(b, mask, 0, 0, stream, true); }
 
 int rg_reset(rg_batch* b, const uint8_t* mask, void* stream) {

@@ -95,6 +95,7 @@ SIGNATURES = {
     "rg_step": (_ci, [_vp, _ci, _ci, _vp]),
     "rg_forward": (_ci, [_vp, _vp]),
     "rg_step_subset": (_ci, [_vp, _vp, _ci, _ci, _vp]),
+    "rg_step_settle": (_ci, [_vp, _vp, _vp, _ci, _cd, _ci, _ci, _vp]),
     "rg_set_const": (_ci, [_vp, _vp, _vp]),
     "rg_reset": (_ci, [_vp, _vp, _vp]),
     "rg_batch_body_aabb": (_ci, [_vp, _vp, _ci, _vp, _vp, _vp, _vp]),
@@ -423,6 +424,20 @@ class BatchedSim:
         else:
             mask = device_mask(self.torch, mask, self.nenv, self.device)
             _check(lib().rg_step_subset(self.h, ptr(mask), nsub, int(final_forward), stream))
+
+    def settle(self, dofs, damping, n_substeps, mask=None, final_forward=True):
+        """`n_substeps` x mj_step with dof_damping = `damping` on the dof ids `dofs` (1 to 64 of them), then `final_forward`
+        x mj_forward with each environment's own damping: the reference's stabilize_objects step loop
+        (robogym/envs/rearrange/common/utils.py:76-93) in one launch for every environment, or with `mask` for the selected
+        ones only (the launch covers just those).  The damping is a launch constant: no per-environment dof_damping row is
+        bound, and neither the model nor a bound row changes (include/robogym_b200.h: rg_step_settle)."""
+        d = np.ascontiguousarray(np.asarray(dofs, dtype=np.int64).ravel())
+        if d.size and (d.min() < np.iinfo(np.int32).min or d.max() > np.iinfo(np.int32).max):
+            raise EngineError("settle: dof id out of range")
+        d = d.astype(np.int32)
+        stream = current_stream(self.torch, self.device)
+        mask = device_mask(self.torch, mask, self.nenv, self.device)
+        _check(lib().rg_step_settle(self.h, ptr(mask), d.ctypes.data, int(d.size), float(damping), int(n_substeps), int(final_forward), stream))
 
     def forward(self, mask=None, count=1):
         if mask is None and count == 1:

@@ -24,6 +24,32 @@ from . import mjcf, rearrange_placement
 GEOM_BOX = 6
 
 
+def object_dofs(m, bodies):
+    """The dof ids of the joints of `bodies` (body_jntadr / body_jntnum), each joint's dofs selected as the reference's
+    get_object_damping does (robogym/envs/rearrange/simulation/base.py:530-546: dof_jntid == the object's joint)."""
+    dof_jntid = np.asarray(m["dof_jntid"])
+    out = []
+    for b in bodies:
+        j0, nj = int(m["body_jntadr"][b]), int(m["body_jntnum"][b])
+        for j in range(j0, j0 + nj):
+            out += np.nonzero(dof_jntid == j)[0].tolist()
+    return out
+
+
+def stabilize_objects(sim, bodies, mask=None, n_steps=100, damping=1e-3):
+    """The reference's stabilize_objects (robogym/envs/rearrange/common/utils.py:76-93, run by every rearrange reset after
+    the objects are placed, base.py:912-913): the objects' dofs get the damping 1e-3, the simulation takes `n_steps` env-steps,
+    the damping is put back and forward() runs.  Here that is one launch of n_steps x sim.n_substeps substeps with the damping
+    as a launch constant (BatchedSim.settle), then the final forward with each environment's own damping, for every
+    environment or those of `mask` (the launch covers just those).
+
+    `bodies` are the object bodies, e.g. BatchedBlockScene.bodies / BatchedMeshScene.bodies.  Every slot's dofs are in the
+    list, the parked ones (unused blocks, empty mesh slots) included: environments are independent and a parked object never
+    touches the table's objects, so the active objects settle as they would without the parked ones in the list."""
+    dofs = object_dofs(sim.model.host, bodies)
+    sim.settle(dofs, damping, int(n_steps) * sim.n_substeps, mask=mask, final_forward=True)
+
+
 class BatchedBlockScene:
     def __init__(self, sim, max_objects=None, prefix="object", park_origin=(3.0, -1.0), park_pitch=0.25):
         self.sim, self.t = sim, sim.torch
