@@ -397,6 +397,56 @@ typedef struct rg_obs_out {
 } rg_obs_out;
 int rg_rearrange_obs(const rg_obs_in* in, const uint8_t* mask_device, const rg_obs_out* out, void* stream);
 
+/* The dual-simulation arm controller's per-step arithmetic (robogym_b200.rearrange_arm.BatchedTcpArmController, TcpSolverMode.
+ * MOCAP_IK): what runs between the solver and main simulations' launches, one thread per selected environment.
+ * rg_arm_tables: the controller's index tables (host struct, passed by value to the kernel).  Ids are checked against the
+ * dims of rg_arm_sim: qpos addresses < nq, actuators < nu, bodies in [1, nbody), mocap slots < nmocap.
+ *   narm arm joints (<= 8): their qpos address in the main and solver models and the main actuator driving each;
+ *   the gripper joint's qpos address and actuator in both; tcp_body: the solver's tool body;
+ *   nweld (1..4) mocap welds of the solver model: mocap slot and welded body; the deltas move the first;
+ *   ndof (1..3) tool rotations: euler_index (0..2, distinct), dof_joint (the arm joint whose range constrains it, -1: none),
+ *   speed (rad per unit action, the mode's speed times max_position_change), lo_lim / hi_lim (the joint's range shrunk by the
+ *   drift threshold); align_axis: -1, or the world axis (0..2) the commanded orientation is re-aligned with;
+ *   max_position_change, grip_lo / grip_hi (the gripper's control range) and grip_half ((grip_hi - grip_lo) / 2).
+ * All arithmetic is float32, each operation rounded as the float32 tensor path rounds it; constants are rounded to float32
+ * where that path converts them. */
+typedef struct rg_arm_tables {
+  int narm;
+  int arm_qpos_main[8]; int arm_qpos_solver[8]; int arm_act_main[8];
+  int grip_qpos_main; int grip_qpos_solver; int grip_act_main; int grip_act_solver;
+  int tcp_body;
+  int nweld; int weld_mocap[4]; int weld_body[4];
+  int ndof; int euler_index[3]; int dof_joint[3];
+  int align_axis;
+  double speed[3]; double lo_lim[8]; double hi_lim[8];
+  double max_position_change; double grip_lo; double grip_hi; double grip_half;
+} rg_arm_tables;
+/* one simulation's rows as the controller reads and writes them (device, float32, row-major per environment): a BatchedSim's
+ * bound qpos [nenv][nq], ctrl [nenv][nu], body_xpos [nenv][nbody][3], body_xquat [nenv][nbody][4], mocap_pos [nenv][nmocap][3],
+ * mocap_quat [nenv][nmocap][4].  The main simulation's body and mocap rows are not read (NULL is fine). */
+typedef struct rg_arm_sim {
+  int nq; int nu; int nbody; int nmocap;
+  float* qpos; float* ctrl; const float* body_xpos; const float* body_xquat; float* mocap_pos; float* mocap_quat;
+} rg_arm_sim;
+/* phase bits of rg_arm_phase; set bits run in this order, each on the environments whose mask byte is set:
+ *   SYNC      solver arm qpos := main arm qpos (arm_reset_controller_error; free_dof_tcp_arm.py:215-226);
+ *   GRIP      solver gripper qpos and ctrl := the main gripper's (on_observations_updated, joint_controlled_tcp_arm.py:129-140);
+ *   SEAT      every weld's mocap body seated on its welded body (gym's reset_mocap2body_xpos);
+ *   PRESOLVE  after the solver's forward: denormalize the action, constrain_quat_ctrl, euler2quat, the TCP quaternion product,
+ *             align_axis, then SEAT and the deltas added to the first weld's mocap body (mocap_set_action);
+ *   POSTSOLVE after the solver's substeps: main arm ctrl := solver arm qpos, main gripper ctrl := the gripper target. */
+enum { RG_ARM_SYNC = 1, RG_ARM_GRIP = 2, RG_ARM_SEAT = 4, RG_ARM_PRESOLVE = 8, RG_ARM_POSTSOLVE = 16 };
+/* `action` (device float32 [nenv][action_dim], action_dim = 3 + ndof + 1) is read by PRESOLVE and POSTSOLVE only (NULL
+ * otherwise).  mask_device: uint8 [mask_len] with mask_len == nenv, or NULL (every environment).  Refuses out-of-range table
+ * ids, a mask of another length and an action width that is not the mode's.  Asynchronous on `stream`. */
+int rg_arm_phase(const rg_arm_tables* tables, int phases, int nenv, const rg_arm_sim* main_sim, const rg_arm_sim* solver_sim, const float* action,
+                 int action_dim, const uint8_t* mask_device, int mask_len, void* stream);
+/* _randomize_robot_initial_position's action_space.sample() for the masked environments: component d of environment e is
+ * numpy's 53-bit double u from Philox4x32-10 keyed by (seed, e) at counter (d, 0, 5, epoch), words (x, y), mapped as gym
+ * 0.15.3's Box.sample maps it for the bounded float32 box [-1, 1]: (float)(-1.0 + 2.0 * u) in fp64.  out: device float32
+ * [nenv][action_dim] (1 <= action_dim <= 8); rows of unselected environments are not written. */
+int rg_arm_sample_actions(int nenv, int action_dim, uint32_t seed, uint32_t epoch, const uint8_t* mask_device, int mask_len, float* out, void* stream);
+
 const char* rg_last_error(void);
 
 #ifdef __cplusplus

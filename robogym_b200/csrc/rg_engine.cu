@@ -22,6 +22,7 @@
 #include "rg_place.inl"
 #include "rg_goal.inl"
 #include "rg_obs.inl"
+#include "rg_arm.inl"
 #include "rg_host.h"
 
 /* The step kernel is built twice.  Registers are granted to a CTA in groups of four warps, so 12 warps (384 threads) may
@@ -239,6 +240,9 @@ __global__ void __launch_bounds__(128) rg_modify_kernel(const __grid_constant__ 
   if (env >= a.nenv || (a.mask && !a.mask[env])) return;
   rg_modify_env(a, (uint32_t)env);
 }
+/* the arm controller's kernels live in rg_arm.cu, compiled without -ftz so that subnormals are kept as torch keeps them */
+cudaError_t rg_arm_launch(const RgArmArgs& a, cudaStream_t stream);
+cudaError_t rg_arm_sample_launch(int nenv, int dim, uint32_t seed, uint32_t epoch, const uint8_t* mask, float* out, cudaStream_t stream);
 /* rg_layout_goals: one warp per selected environment */
 __global__ void __launch_bounds__(128) rg_layout_kernel(const __grid_constant__ RgLayoutArgs a) {
   const int env = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -959,6 +963,25 @@ int rg_rearrange_obs(const rg_obs_in* in, const uint8_t* mask, const rg_obs_out*
   if (err) return rg_fail(-1, std::string("rg_rearrange_obs: ") + err);
   rg_obs_kernel<<<(a.in.nenv + 3) / 4, 128, 0, (cudaStream_t)stream>>>(a);
   RG_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int rg_arm_phase(const rg_arm_tables* tables, int phases, int nenv, const rg_arm_sim* main_sim, const rg_arm_sim* solver_sim, const float* action,
+                 int action_dim, const uint8_t* mask, int mask_len, void* stream) {
+  const char* err = rg_arm_check(tables, phases, nenv, main_sim, solver_sim, action, action_dim, mask, mask_len);
+  if (err) return rg_fail(-1, std::string("rg_arm_phase: ") + err);
+  RgArmArgs a;
+  a.t = *tables; a.main = *main_sim; a.solver = *solver_sim;
+  a.phases = phases; a.nenv = nenv; a.action_dim = action_dim; a.action = action; a.mask = mask;
+  RG_CUDA(rg_arm_launch(a, (cudaStream_t)stream));
+  return 0;
+}
+
+int rg_arm_sample_actions(int nenv, int action_dim, uint32_t seed, uint32_t epoch, const uint8_t* mask, int mask_len, float* out, void* stream) {
+  if (nenv <= 0 || !out) return rg_fail(-1, "rg_arm_sample_actions: bad argument");
+  if (action_dim < 1 || action_dim > RG_ARM_MAXACT) return rg_fail(-1, "rg_arm_sample_actions: action_dim must be 1..8");
+  if (mask && mask_len != nenv) return rg_fail(-1, "rg_arm_sample_actions: the mask must hold one byte per environment (mask_len == nenv)");
+  RG_CUDA(rg_arm_sample_launch(nenv, action_dim, seed, epoch, mask, out, (cudaStream_t)stream));
   return 0;
 }
 }

@@ -64,6 +64,24 @@ class ObsOut(ctypes.Structure):
         "sim_reward sim_done").split()]
 
 
+class ArmTables(ctypes.Structure):
+    """rg_arm_tables (include/robogym_b200.h)"""
+    _fields_ = [("narm", _ci), ("arm_qpos_main", _ci * 8), ("arm_qpos_solver", _ci * 8), ("arm_act_main", _ci * 8), ("grip_qpos_main", _ci),
+                ("grip_qpos_solver", _ci), ("grip_act_main", _ci), ("grip_act_solver", _ci), ("tcp_body", _ci), ("nweld", _ci), ("weld_mocap", _ci * 4),
+                ("weld_body", _ci * 4), ("ndof", _ci), ("euler_index", _ci * 3), ("dof_joint", _ci * 3), ("align_axis", _ci), ("speed", _cd * 3),
+                ("lo_lim", _cd * 8), ("hi_lim", _cd * 8), ("max_position_change", _cd), ("grip_lo", _cd), ("grip_hi", _cd), ("grip_half", _cd)]
+
+
+class ArmSim(ctypes.Structure):
+    """rg_arm_sim (include/robogym_b200.h)"""
+    _fields_ = [("nq", _ci), ("nu", _ci), ("nbody", _ci), ("nmocap", _ci), ("qpos", _vp), ("ctrl", _vp), ("body_xpos", _vp), ("body_xquat", _vp),
+                ("mocap_pos", _vp), ("mocap_quat", _vp)]
+
+
+# rg_arm_phase phase bits
+ARM_SYNC, ARM_GRIP, ARM_SEAT, ARM_PRESOLVE, ARM_POSTSOLVE = 1, 2, 4, 8, 16
+
+
 # name -> (restype, argtypes) of every function include/robogym_b200.h declares, in its order (tests/test_abi.py checks the
 # table against the header)
 SIGNATURES = {
@@ -105,6 +123,8 @@ SIGNATURES = {
     "rg_rearrange_goal": (_ci, [_P(GoalIn), _vp, _vp, _P(GoalOut), _vp]),
     "rg_goal_orientations": (_ci, [_ci, _ci, _vp, _vp, _ci, _u32, _u32, _vp, _vp, _vp]),
     "rg_rearrange_obs": (_ci, [_P(ObsIn), _vp, _P(ObsOut), _vp]),
+    "rg_arm_phase": (_ci, [_P(ArmTables), _ci, _ci, _P(ArmSim), _P(ArmSim), _vp, _ci, _vp, _ci, _vp]),
+    "rg_arm_sample_actions": (_ci, [_ci, _ci, _u32, _u32, _vp, _ci, _vp, _vp]),
     "rg_last_error": (_str, []),
 }
 

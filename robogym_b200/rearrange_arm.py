@@ -18,10 +18,17 @@ driven by mujoco-py's cascaded-PI controllers, tracks them.  Per env-step (robog
      (robot_env.py:677) -- mujoco-py's controller state advances in each forward, so the count matters (`main_forwards`)
   4. `on_observations_updated` (joint_controlled_tcp_arm.py:129-140): the solver's gripper follows the main gripper
 
-Here both simulations are `BatchedSim`s (one fused launch each per env-step) and steps 1-4 are a few tensor ops between the two
-launches; nothing leaves the device.  The class works on any object with BatchedSim's attributes, so the CPU tier runs it on the
-oracle stand-in (tests/stubs) beside the unmodified reference environment (tests/test_rearrange_arm.py).
+Here both simulations are `BatchedSim`s (one fused launch each per env-step) and steps 1-4 are one masked kernel launch
+between each pair of simulation launches (rg_arm_phase, csrc/rg_arm.inl); nothing leaves the device.  The class also works on
+any object with BatchedSim's attributes on the CPU: there steps 1-4 are the float tensor ops of `_step_torch`, so the CPU tier
+runs it on the oracle stand-in (tests/stubs) beside the unmodified reference environment (tests/test_rearrange_arm.py), and the
+GPU tests hold the kernel to that path bit for bit.
+
+The robot's part of the reference's reset is here too: `initialize_sim_state` (RearrangeEnv._initialize_sim_state for MOCAP_IK,
+rearrange/common/base.py:448-465) and `randomize_initial_position` (_randomize_robot_initial_position, :484-496: one random
+action held for n_random_initial_steps env-steps, then zero actions), for the environments of a mask.
 """
+import ctypes
 import math
 
 import numpy as np
@@ -32,6 +39,7 @@ EULER_INDEX = {"roll": 0, "pitch": 2, "yaw": 1}
 JOINT_OF_DOF = {"pitch": 5}                      # MocapSolver.JOINT_MAPPING (mocap_solver.py:17-19)
 JOINT_DRIFT_THRESHOLD = math.radians(1)         # free_dof_tcp_arm.py:26-28
 EQ_WELD = 1
+TABLETOP_EXPERIMENT_INITIAL_POS = np.deg2rad([135.0, -90.0, 135.0, -100.0, -240.0, 135.0])   # robot/ur16e/arm_interface.py:27
 
 
 def euler2quat(t, euler):
@@ -124,16 +132,85 @@ class BatchedTcpArmController:
         self.jnt_hi = [float(jr[j, 1]) for j in self.arm_jnt_solver]
         self.speed = [DOF_SPEED[d] * self.max_position_change for d in self.dof_dims]
         self.action_dim = 3 + len(self.dof_dims) + 1
+        # CUDA simulations run steps 1-4 as the kernel of rg_arm_phase, from these tables (built once, passed with every launch)
+        self.on_device = bool(getattr(main.qpos, "is_cuda", False))
+        self._tables = self._arm_tables() if self.on_device else None
+        # configurations whose kernel steps are bit-identical to the tensor path's (DESIGN §9): in the others an unmasked step()
+        # keeps the tensor path, so what it computes does not change; masked steps and the reset run the kernel everywhere
+        self.kernel_exact = self.on_device and self.align_axis is None
+
+    def _arm_tables(self):
+        from . import engine
+
+        T = engine.ArmTables()
+        T.narm = len(self.arm_qadr_main)
+        for j in range(T.narm):
+            T.arm_qpos_main[j], T.arm_qpos_solver[j], T.arm_act_main[j] = self.arm_qadr_main[j], self.arm_qadr_solver[j], self.arm_act_main[j]
+            T.lo_lim[j] = self.jnt_lo[j] + JOINT_DRIFT_THRESHOLD           # the scalars constrain_quat_ctrl subtracts the joint from
+            T.hi_lim[j] = self.jnt_hi[j] - JOINT_DRIFT_THRESHOLD
+        T.grip_qpos_main, T.grip_qpos_solver, T.grip_act_main, T.grip_act_solver = self.grip_qadr_main, self.grip_qadr_solver, self.grip_act_main, self.grip_act_solver
+        T.tcp_body = self.tcp_body
+        T.nweld = len(self.welds)
+        for w, (_, k, body) in enumerate(self.welds):
+            T.weld_mocap[w], T.weld_body[w] = k, body
+        T.ndof = len(self.dof_dims)
+        for i, d in enumerate(self.dof_dims):
+            T.euler_index[i] = EULER_INDEX[d]
+            T.dof_joint[i] = JOINT_OF_DOF.get(d, -1)
+            T.speed[i] = self.speed[i]
+        T.align_axis = -1 if self.align_axis is None else self.align_axis
+        T.max_position_change, T.grip_lo, T.grip_hi = self.max_position_change, self.grip_lo, self.grip_hi
+        T.grip_half = (self.grip_hi - self.grip_lo) / 2.0
+        return T
+
+    @staticmethod
+    def _arm_sim(sim):
+        from . import engine
+
+        m = sim.model.host
+        return engine.ArmSim(int(m["nq"]), int(m["nu"]), int(m["nbody"]), int(m["nmocap"]), *[engine.ptr(getattr(sim, n, None)) for n in
+                             ("qpos", "ctrl", "body_xpos", "body_xquat", "mocap_pos", "mocap_quat")])
+
+    def _phase(self, phases, mask, action=None):
+        """one launch of rg_arm_phase on the environments of `mask` (a device uint8 tensor, or None: all)"""
+        from . import engine
+
+        if action is not None:
+            if tuple(action.shape) != (self.main.nenv, self.action_dim):
+                raise ValueError(f"action: expected shape {(self.main.nenv, self.action_dim)}, got {tuple(action.shape)}")
+            action = action.to(device=self.main.device, dtype=self.t.float32).contiguous()
+        width = self.action_dim
+        engine._check(engine.lib().rg_arm_phase(ctypes.byref(self._tables), int(phases), self.main.nenv, ctypes.byref(self._arm_sim(self.main)),
+                                                ctypes.byref(self._arm_sim(self.solver)), engine.ptr(action), width, engine.ptr(mask),
+                                                0 if mask is None else int(mask.numel()), engine.current_stream(self.t, self.main.device)))
+
+    def _mask(self, mask):
+        from . import engine
+
+        if not self.on_device:
+            if mask is not None:
+                raise ValueError("a mask needs the CUDA simulations; the tensor path steps every environment")
+            return None
+        return engine.device_mask(self.t, mask, self.main.nenv, self.main.device)
 
     # ---- reset: JointControlledTcpArm.__init__ / reset (joint_controlled_tcp_arm.py:52-58,100-102), MocapSolver.reset (mocap_solver.py:55-57)
-    def reset(self):
+    def reset(self, mask=None):
         """Call after the main simulation has its initial state: the solver arm takes the main arm's joint angles and its gripper
-        state, the mocap welds are re-zeroed (relative pose = identity) and the mocap bodies seated on the tool."""
+        state, the mocap welds are re-zeroed (relative pose = identity, model-wide) and the mocap bodies seated on the tool.
+        `mask` ([nenv] bool / uint8; CUDA simulations only): only those environments."""
         ms = self.solver.model.host
         data = np.array(ms["eq_data"], dtype=np.float64).reshape(int(ms["neq"]), -1)
         for i, _, _ in self.welds:
             data[i, :7] = [0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0]
         self.solver.model.set_field("eq_data", data.reshape(-1))
+        mask = self._mask(mask)
+        if self.on_device:
+            from . import engine
+
+            self._phase(engine.ARM_SYNC | engine.ARM_GRIP, mask)
+            self.solver.forward(mask)
+            self._phase(engine.ARM_SEAT, mask)
+            return
         self.solver.qpos[:, self.arm_qadr_solver] = self.main.qpos[:, self.arm_qadr_main].to(self.solver.qpos.dtype)
         self.solver.qpos[:, self.grip_qadr_solver] = self.main.qpos[:, self.grip_qadr_main].to(self.solver.qpos.dtype)
         self.solver.ctrl[:, self.grip_act_solver] = self.main.ctrl[:, self.grip_act_main].to(self.solver.ctrl.dtype)
@@ -188,9 +265,105 @@ class BatchedTcpArmController:
         self.main.ctrl[:, self.grip_act_main] = grip.to(self.main.ctrl.dtype)
 
     # ---- steps 1-4
-    def step(self, action):
+    def step(self, action, mask=None):
+        """One env-step: the action ([nenv, action_dim] in [-1, 1]) through the solver simulation into the main simulation's
+        controls, the main simulation's step with `main_forwards` forwards, the solver's gripper synced.  `mask` ([nenv] bool /
+        uint8; CUDA simulations only): only those environments are stepped, the others are left as they are."""
+        if mask is None and not self.kernel_exact:
+            return self._step_torch(action, self.main_forwards)
+        self._step(action, self._mask(mask), self.main_forwards, True)
+
+    def _step(self, action, mask, main_forwards, grip_sync, main_step=True):
+        if not self.on_device:
+            return self._step_torch(action, main_forwards, grip_sync, main_step)
+        from . import engine
+
+        if self.reset_controller_error:
+            self._phase(engine.ARM_SYNC, mask)
+            self.solver.forward(mask)
+        self._phase(engine.ARM_PRESOLVE, mask, action)
+        self.solver.step(final_forward=0, mask=mask)
+        self._phase(engine.ARM_POSTSOLVE, mask, action)
+        if main_step:
+            self.main.step(final_forward=main_forwards, mask=mask)
+            if grip_sync:
+                self._phase(engine.ARM_GRIP, mask)
+
+    def _step_torch(self, action, main_forwards, grip_sync=True, main_step=True):
+        """steps 1-4 as float tensor ops, every environment: the path of the CPU stand-ins, and the reference the GPU tests hold
+        the kernel to"""
         pos, ang, grip = self.denormalize(action)
         self.set_position_control(pos, ang, grip)
-        self.main.step(final_forward=self.main_forwards)
-        self.solver.qpos[:, self.grip_qadr_solver] = self.main.qpos[:, self.grip_qadr_main].to(self.solver.qpos.dtype)
-        self.solver.ctrl[:, self.grip_act_solver] = self.main.ctrl[:, self.grip_act_main].to(self.solver.ctrl.dtype)
+        if not main_step:
+            return
+        self.main.step(final_forward=main_forwards)
+        if grip_sync:
+            self.solver.qpos[:, self.grip_qadr_solver] = self.main.qpos[:, self.grip_qadr_main].to(self.solver.qpos.dtype)
+            self.solver.ctrl[:, self.grip_act_solver] = self.main.ctrl[:, self.grip_act_main].to(self.solver.ctrl.dtype)
+
+    # ---- the robot's part of the reset (RearrangeEnv._reset, rearrange/common/base.py:897-932)
+    def initialize_sim_state(self, mask=None):
+        """_initialize_sim_state for TcpSolverMode.MOCAP_IK (base.py:448-465): the main simulation's welds switched off
+        (model-wide), then robot.reset(): the main arm at TABLETOP_EXPERIMENT_INITIAL_POS in qpos and ctrl
+        (JointControlledArm.set_simulation_start_position, joint_controlled_arm.py:123-132) and the controller's reset.  The
+        reference rebuilds both simulations before this (_recreate_sim), so velocities, controller (PID) state and warm starts
+        of both are cleared here; the rebuilt solver arm already stands at the start pose, which is what reset()'s copy of the
+        main arm gives it.  The reference calls this before the objects are placed and settled (base.py:904-913)."""
+        dev_mask = self._mask(mask)                     # refused before anything is written
+        t = self.t
+        keep = None if mask is None else (~t.as_tensor(mask, device=self.main.qpos.device).reshape(-1, 1).bool())
+        for sim in (self.main, self.solver):            # _recreate_sim: both simulations start at rest, controller state cleared
+            for name in ("qvel", "pid", "qacc_warmstart"):
+                v = getattr(sim, name)
+                if keep is None:
+                    v.zero_()
+                else:
+                    v.mul_(keep.to(v.dtype))
+        mm = self.main.model.host
+        active = np.array(mm["eq_active"]).reshape(-1).copy()
+        active[np.asarray(mm["eq_type"]).reshape(-1) == EQ_WELD] = 0
+        self.main.model.set_field("eq_active", active)
+        start = self.t.tensor(TABLETOP_EXPERIMENT_INITIAL_POS, dtype=self.main.qpos.dtype, device=self.main.qpos.device)
+        if mask is None:
+            self.main.qpos[:, self.arm_qadr_main] = start
+            self.main.ctrl[:, self.arm_act_main] = start.to(self.main.ctrl.dtype)
+        else:
+            self.main.qpos[:, self.arm_qadr_main] = t.where(keep, self.main.qpos[:, self.arm_qadr_main], start)
+            self.main.ctrl[:, self.arm_act_main] = t.where(keep, self.main.ctrl[:, self.arm_act_main], start.to(self.main.ctrl.dtype))
+        self.reset(dev_mask)
+
+    def sample_initial_action(self, seed, epoch, mask=None):
+        """action_space.sample() of each environment of `mask` on the device ([nenv, action_dim] float32; rows of other
+        environments are zero): Philox4x32-10 keyed by (seed, environment) under purpose 5, gym's Box.sample mapping (rg_arm_sample_actions)"""
+        from . import engine
+
+        if not self.on_device:
+            raise ValueError("sample_initial_action draws on the CUDA device; on other simulations pass the action to hold_initial_action")
+        t = self.t
+        m = engine.device_mask(t, mask, self.main.nenv, self.main.device)
+        out = t.zeros(self.main.nenv, self.action_dim, dtype=t.float32, device=self.main.device)
+        engine._check(engine.lib().rg_arm_sample_actions(self.main.nenv, self.action_dim, int(seed) & 0xFFFFFFFF, int(epoch) & 0xFFFFFFFF, engine.ptr(m),
+                                                         0 if m is None else int(m.numel()), engine.ptr(out), engine.current_stream(t, self.main.device)))
+        return out
+
+    def hold_initial_action(self, action, mask=None, n_random_initial_steps=10, n_zero_steps=100):
+        """the step loop of _randomize_robot_initial_position (base.py:484-496) with a given action: n_random_initial_steps
+        env-steps of `action`, one controller step of the zero action without a main step, then n_zero_steps env-steps of the zero
+        action.  Each env-step is _set_action and mujoco_simulation.step(): ONE main forward and no gripper sync, as the
+        reference has no observation between them.  With n_random_initial_steps < 1 nothing is stepped."""
+        if n_random_initial_steps < 1:
+            return
+        mask = self._mask(mask)
+        for _ in range(int(n_random_initial_steps)):
+            self._step(action, mask, 1, False)
+        zero = action * 0.0
+        self._step(zero, mask, 1, False, main_step=False)
+        for _ in range(int(n_zero_steps)):
+            self._step(zero, mask, 1, False)
+
+    def randomize_initial_position(self, mask, seed, epoch, n_random_initial_steps=10, n_zero_steps=100):
+        """_randomize_robot_initial_position for the environments of `mask` (None: all): the held random action is drawn on the
+        device (sample_initial_action) and returned."""
+        action = self.sample_initial_action(seed, epoch, mask)
+        self.hold_initial_action(action, mask, n_random_initial_steps, n_zero_steps)
+        return action
