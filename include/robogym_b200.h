@@ -447,6 +447,45 @@ int rg_arm_phase(const rg_arm_tables* tables, int phases, int nenv, const rg_arm
  * [nenv][action_dim] (1 <= action_dim <= 8); rows of unselected environments are not written. */
 int rg_arm_sample_actions(int nenv, int action_dim, uint32_t seed, uint32_t epoch, const uint8_t* mask_device, int mask_len, float* out, void* stream);
 
+/* The object groups of a rearrange reset, one thread per selected environment: RearrangeEnv._sample_random_object_groups
+ * (with sample_group_counts), _sample_group_attributes and _sample_default_quaternions (robogym/envs/rearrange/common/
+ * base.py:513-620, common/utils.py:47-73) and their overrides in blocks.py, blocks_duplicate.py, the dedupe environments,
+ * holdout.py, common/mesh.py and ycb.py.  Environment e's objects are its first active[e] slots; its groups take them in
+ * order.  Every input is HOST memory (the call copies what the kernel reads).
+ *   active: int32 [nenv], each in [0, nobj] (nobj <= 64);
+ *   group_mode: 1 random (sample_group_counts with lam ~ uniform(lam_low, lam_high)), 2 dedupe (every object its own group,
+ *     no draws), 3 single (blocks_duplicate: the random counts drawn, then one group of all), 4 fixed (fixed_counts int32
+ *     [nenv][nobj]: each row positive counts summing to the active count, then zeros, as holdout's task_object_configs);
+ *   per group: a material index in [0, n_materials) (n_materials >= 1: choice(material_names)); a colour, color_mode 1 random
+ *     (random((g, 4)), alpha 1), 2 palette (permutation(palette)[:g]; palette fp64 [n_palette][4], n_palette in
+ *     [largest active count, 256]) or 3 grey ((0.5, 0.5, 0.5, 1), no draws); a size scale exp(uniform(-scale_low,
+ *     scale_high)); with mesh_mode 1 (with replacement) or 2 (without: permutation(n_candidates)[:g], n_candidates <= 256 and
+ *     no environment with more possible groups than candidates) a candidate index in [0, n_candidates), n_candidates >= 1;
+ *   per object: the yaw uniform(0, 2 pi) and its quaternion about z (w, x, y, z).
+ * Random numbers: Philox4x32-10 keyed by (seed, e); the groups and attributes take counter (d, 0, 6, epoch) for their d-th
+ * draw in the reference's call order, object j's yaw counter (j, 1, 6, epoch) (robogym_b200/csrc/rg_groups.inl lists the
+ * order).  Outputs (device, [nenv][nobj] row-major; rgba and quat [nenv][nobj][4]): group (the group id, 0-based in slot
+ * order, the `group` of rg_goal_in), count (the group's size), material, rgba, scale, mesh (-1 without mesh draws), yaw,
+ * quat; ngroups [nenv].  Slots past an environment's objects get -1 (group, material, mesh) or 0 (the rest).  Unselected
+ * environments (mask_device: uint8 [mask_len], mask_len == nenv, or NULL) are not written.  Refuses more than 64 objects,
+ * active counts outside [0, nobj], a non-finite lam or scale range, n_materials < 1, a palette with fewer rows than the
+ * largest active count, mesh draws without candidates, more groups than candidates without replacement and a mask of
+ * another length.  Asynchronous on `stream`; the host inputs are staged before the call returns, so the caller may reuse them. */
+typedef struct rg_groups_in {
+  int nenv; int nobj;
+  const int* active;
+  int group_mode; double lam_low; double lam_high; const int* fixed_counts;
+  int n_materials;
+  int color_mode; const double* palette; int n_palette;
+  double scale_low; double scale_high;
+  int mesh_mode; int n_candidates;
+  uint32_t seed; uint32_t epoch;
+} rg_groups_in;
+typedef struct rg_groups_out {
+  int* group; int* count; int* material; double* rgba; double* scale; int* mesh; double* yaw; double* quat; int* ngroups;
+} rg_groups_out;
+int rg_object_groups(const rg_groups_in* in, const uint8_t* mask_device, int mask_len, const rg_groups_out* out, void* stream);
+
 const char* rg_last_error(void);
 
 #ifdef __cplusplus

@@ -7,12 +7,13 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "librobogym_b200.so")
-DEPS = [os.path.join(SRC, f) for f in ("rg_engine.cu", "rg_cta.cu", "rg_arm.cu", "rg_kernel.inl", "rg_defs.h", "rg_dyn.inl", "rg_col.inl", "rg_sol.inl", "rg_step.inl", "rg_place.inl", "rg_goal.inl", "rg_obs.inl", "rg_arm.inl", "rg_host.h", "rg_derived_fields.h")]
+DEPS = [os.path.join(SRC, f) for f in ("rg_engine.cu", "rg_cta.cu", "rg_arm.cu", "rg_groups.cu", "rg_kernel.inl", "rg_defs.h", "rg_dyn.inl", "rg_col.inl", "rg_sol.inl", "rg_step.inl", "rg_place.inl", "rg_goal.inl", "rg_obs.inl", "rg_arm.inl", "rg_groups.inl", "rg_host.h", "rg_derived_fields.h")]
 DEPS += [os.path.join(HERE, "..", "include", f) for f in ("rg_model_fields.h", "robogym_b200.h")]
 
 
-# the one-warp kernel (rg_engine.cu, with the C ABI) and the one-environment-per-CTA kernel (rg_cta.cu), linked into one library
-SOURCES = ("rg_engine.cu", "rg_cta.cu")
+# the one-warp kernel (rg_engine.cu, with the C ABI), the one-environment-per-CTA kernel (rg_cta.cu) and the object groups'
+# kernel (rg_groups.cu), linked into one library
+SOURCES = ("rg_engine.cu", "rg_cta.cu", "rg_groups.cu")
 
 
 def nvcc_cmd(extra=(), sources=("rg_engine.cu",), objects=()):

@@ -243,6 +243,8 @@ __global__ void __launch_bounds__(128) rg_modify_kernel(const __grid_constant__ 
 /* the arm controller's kernels live in rg_arm.cu, compiled without -ftz so that subnormals are kept as torch keeps them */
 cudaError_t rg_arm_launch(const RgArmArgs& a, cudaStream_t stream);
 cudaError_t rg_arm_sample_launch(int nenv, int dim, uint32_t seed, uint32_t epoch, const uint8_t* mask, float* out, cudaStream_t stream);
+/* the object groups' kernel lives in rg_groups.cu: argument checks and launch (nullptr), or what is wrong with the arguments */
+const char* rg_groups_run(const rg_groups_in* in, const uint8_t* mask, int mask_len, const rg_groups_out* out, cudaStream_t stream, cudaError_t* err);
 /* rg_layout_goals: one warp per selected environment */
 __global__ void __launch_bounds__(128) rg_layout_kernel(const __grid_constant__ RgLayoutArgs a) {
   const int env = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -982,6 +984,14 @@ int rg_arm_sample_actions(int nenv, int action_dim, uint32_t seed, uint32_t epoc
   if (action_dim < 1 || action_dim > RG_ARM_MAXACT) return rg_fail(-1, "rg_arm_sample_actions: action_dim must be 1..8");
   if (mask && mask_len != nenv) return rg_fail(-1, "rg_arm_sample_actions: the mask must hold one byte per environment (mask_len == nenv)");
   RG_CUDA(rg_arm_sample_launch(nenv, action_dim, seed, epoch, mask, out, (cudaStream_t)stream));
+  return 0;
+}
+
+int rg_object_groups(const rg_groups_in* in, const uint8_t* mask, int mask_len, const rg_groups_out* out, void* stream) {
+  cudaError_t e = cudaSuccess;
+  const char* err = rg_groups_run(in, mask, mask_len, out, (cudaStream_t)stream, &e);
+  if (err) return rg_fail(-1, std::string("rg_object_groups: ") + err);
+  RG_CUDA(e);
   return 0;
 }
 }

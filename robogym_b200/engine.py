@@ -82,6 +82,18 @@ class ArmSim(ctypes.Structure):
 ARM_SYNC, ARM_GRIP, ARM_SEAT, ARM_PRESOLVE, ARM_POSTSOLVE = 1, 2, 4, 8, 16
 
 
+class GroupsIn(ctypes.Structure):
+    """rg_groups_in (include/robogym_b200.h)"""
+    _fields_ = [("nenv", _ci), ("nobj", _ci), ("active", _vp), ("group_mode", _ci), ("lam_low", _cd), ("lam_high", _cd), ("fixed_counts", _vp),
+                ("n_materials", _ci), ("color_mode", _ci), ("palette", _vp), ("n_palette", _ci), ("scale_low", _cd), ("scale_high", _cd),
+                ("mesh_mode", _ci), ("n_candidates", _ci), ("seed", _u32), ("epoch", _u32)]
+
+
+class GroupsOut(ctypes.Structure):
+    """rg_groups_out (include/robogym_b200.h)"""
+    _fields_ = [(k, _vp) for k in "group count material rgba scale mesh yaw quat ngroups".split()]
+
+
 # name -> (restype, argtypes) of every function include/robogym_b200.h declares, in its order (tests/test_abi.py checks the
 # table against the header)
 SIGNATURES = {
@@ -125,6 +137,7 @@ SIGNATURES = {
     "rg_rearrange_obs": (_ci, [_P(ObsIn), _vp, _P(ObsOut), _vp]),
     "rg_arm_phase": (_ci, [_P(ArmTables), _ci, _ci, _P(ArmSim), _P(ArmSim), _vp, _ci, _vp, _ci, _vp]),
     "rg_arm_sample_actions": (_ci, [_ci, _ci, _u32, _u32, _vp, _ci, _vp, _vp]),
+    "rg_object_groups": (_ci, [_P(GroupsIn), _vp, _ci, _P(GroupsOut), _vp]),
     "rg_last_error": (_str, []),
 }
 
